@@ -36,7 +36,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 ALG_BYTES_NOTE = "refLen + readLen + n*n + 40 bytes per pair (SURVEY 8(d))"
 METRIC = "GCUPS (DP cell updates/s), ssw_align forward path"
 CONFIG_NOTES = {
-    "l2": "b200 arm: a 256 MB buffer is written between timed steps (L2 flush) and every step streams its own scratch; reference arm: CPU, n/a",
+    "l2": "b200 arm: a 256 MB buffer (> the 50 MB L2 of an H100) is written between timed steps (L2 flush) and every step streams its own scratch; reference arm: CPU, n/a",
     "timing": "b200 arm: per step max(CUDA-event time on the engine stream, wall clock between synchronised barriers), max over ranks; "
               "reference arm: wall clock of the pthread harness over a bounded sample of the same read set (a rate)",
 }
@@ -51,7 +51,7 @@ def parse():
     ap.add_argument("--reads", type=int, default=100_000, help="reads of the headline batch (config 3: 100,000)")
     ap.add_argument("--only", default="3,2,4,5", help="shapes to run, e.g. 3,2 (3 is the headline and always runs)")
     ap.add_argument("--e2e-reps", type=int, default=2, help="timed end-to-end repetitions per shape")
-    ap.add_argument("--sub-steps", type=int, default=3, help="timed steps of the sub-result shapes (configs 2, 4, 5)")
+    ap.add_argument("--sub-steps", type=int, default=None, help="timed steps of the sub-result shapes (configs 2, 4, 5; default: --steps)")
     ap.add_argument("--c4-queries", type=int, default=512, help="queries of the config-4 slice (of 10,000) x all 50,000 targets")
     ap.add_argument("--c4-targets", type=int, default=50_000)
     ap.add_argument("--parity", type=int, default=256, help="gathered config-3 records re-computed by the CPU reference (untimed)")
@@ -64,7 +64,13 @@ def parse():
     ap.add_argument("--dry-run-emu", action="store_true",
                     help="tests only: run the orchestration on the CPU emulator build of the kernels (tests/cuda_emu) with tiny shapes and "
                          "the gloo backend; the printed line is marked dry_run and its numbers mean nothing")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the records each shape returned in its last timed call (the last end-to-end repetition, or the last "
+                         "resident step with --e2e-reps 0) to DIR/<shape>_<field>.npy (see dump_outputs)")
+    args = ap.parse_args()
+    if args.sub_steps is None:
+        args.sub_steps = args.steps
+    return args
 
 
 def workload_name(n_reads):
@@ -76,8 +82,8 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         with open(p) as f:
-            return json.load(f).get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+            return json.load(f).get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json hbm_gbs)"
+    return 3350.0, "fallback: H100 SXM data sheet (HBM3, 700 W card)"
 
 
 class ClockSampler:
@@ -243,7 +249,9 @@ def shard_of(W, cfg, D, rank, world):
 
 
 def run_shape(X, cfg, W, steps, warmup, e2e_reps, sampler=None):
-    """Time one shape.  Returns (stats dict on every rank, gathered records + pool on rank 0)."""
+    """Time one shape: `steps` resident steps, then `e2e_reps` end-to-end repetitions (a separate measurement, see --e2e-reps).
+    Returns (stats dict on every rank, gathered records + pool on rank 0 of the last timed call: the last end-to-end
+    repetition, or the last resident step when e2e_reps is 0; both align the same inputs with the same parameters)."""
     import torch
     import torch.distributed as dist
     D, L, eng = X.D, X.L, X.eng
@@ -348,9 +356,33 @@ def parity_check(W, got, n_check, n_r):
             "first_bad_pairs": [int(idx[i]) for i in bad[:4]]}
 
 
+DUMP_FIELDS = ("score1", "score2", "ref_begin1", "ref_end1", "read_begin1", "read_end1", "ref_end2", "flag", "status", "cigar_len")
+DUMP_MAX_RECORDS = 500_000          # 10 fields x 4 B: config 4's 25.6 M records are sampled to keep the whole dump under 64 MB
+
+
+def dump_outputs(out_dir, shape, got):
+    """Write the records gathered in the last timed call of `shape` (what run_shape returns: the last end-to-end repetition,
+    or the last resident step with --e2e-reps 0) as <shape>_<field>.npy (float32: every value is an integer
+    below 2^24, so exact) and, for shapes that compute CIGARs (flag & 7), the CIGAR words of those records, concatenated in
+    record order, as <shape>_cigar.npy (float64); score-only shapes return no CIGAR words, so they have no such file.
+    Record sets larger than DUMP_MAX_RECORDS are reduced to a fixed, seeded sample; <shape>_pair_index.npy names its pairs."""
+    recs, pool = got
+    idx = np.arange(len(recs))
+    if len(recs) > DUMP_MAX_RECORDS:
+        idx = np.sort(np.random.default_rng(0).choice(len(recs), DUMP_MAX_RECORDS, replace=False))
+    os.makedirs(out_dir, exist_ok=True)
+    sel = recs[idx]
+    np.save(os.path.join(out_dir, shape + "_pair_index.npy"), idx.astype(np.float64))
+    for f in DUMP_FIELDS:
+        np.save(os.path.join(out_dir, "%s_%s.npy" % (shape, f)), sel[f].astype(np.float32))
+    words = [pool[o: o + n] for o, n in zip(sel["cigar_off"].tolist(), sel["cigar_len"].tolist()) if n > 0 and o >= 0]
+    if words:
+        np.save(os.path.join(out_dir, shape + "_cigar.npy"), np.concatenate(words).astype(np.float64))
+
+
 def alu_roofline(cells, fill_s):
     """Cell updates/s of the fill kernels against the measured DPX issue peak (profiles/dpx_peak.json, written by
-    tools/microbench on the B200): 5.5 packed-s16x2 ops per 2 cells."""
+    tools/microbench on an H100): 5.5 packed-s16x2 ops per 2 cells."""
     p = os.path.join(ROOT, "profiles", "dpx_peak.json")
     peak = None
     if os.path.exists(p):
@@ -358,7 +390,7 @@ def alu_roofline(cells, fill_s):
             peak = json.load(f).get("gcups_peak_5p5_ops_per_cellpair")
     ach = cells / fill_s / 1e9 if fill_s > 0 else None
     return {"achieved_gcups": ach, "peak_gcups": peak, "frac": (ach / peak) if (peak and ach) else None,
-            "unit": "GCUPS", "basis": "measured VIADDMNMX.S16x2 issue rate x 148 SMs / 2.75 ops per cell"}
+            "unit": "GCUPS", "basis": "measured VIADDMNMX.S16x2 issue rate x the SMs of the device / 2.75 ops per cell"}
 
 
 def sub_result(st, world, name, what, extra=None):
@@ -372,8 +404,7 @@ def sub_result(st, world, name, what, extra=None):
         # slices on helper streams: their fill times are taken while they share the device and add up to more than the step
         o["alu_roofline"] = alu_roofline(st["cells"] / world, st["step_ms"] * 1e-3)
         o["alu_roofline"]["basis"] += ("; denominator = the whole step (forward fills of concurrent slices overlap with reverse fills and tracebacks, "
-                                       "their summed times exceed the step): a lower bound of the fill kernels' own efficiency "
-                                       "(kernel alone: profiles/ncu_strips_cfg5_r2.txt)")
+                                       "their summed times exceed the step): a lower bound of the fill kernels' own efficiency")
     if extra:
         o.update(extra)
     return o
@@ -419,7 +450,7 @@ def main():
     for kv in args.opt:
         name, val = kv.split("=")
         X.eng.set_option(name, int(val))
-    X.flush = torch.empty((1 << 10) if X.emu else (256 << 20), dtype=torch.uint8, device=X.dev)       # > 126 MB L2
+    X.flush = torch.empty((1 << 10) if X.emu else (256 << 20), dtype=torch.uint8, device=X.dev)       # > 50 MB L2
     only = set(int(x) for x in args.only.split(",") if x.strip())
     rank0 = X.rank == 0
     do_cpu = rank0 and X.world == 1 and not args.no_cpu_baseline
@@ -439,16 +470,7 @@ def main():
         fl = max(st3["fill_launches_per_step_all_ranks"] / X.world, 1.0)                                  # launches per rank and step
         fill_s = max(st3["fill_ms"] * 1e-3, 1e-9)
         achieved = alg_bytes_step / fill_s / 1e9
-        traffic, traffic_src = None, None
-        tp = os.path.join(ROOT, "profiles", "traffic_fill.json")
-        if os.path.exists(tp):
-            with open(tp) as f:
-                tj = json.load(f)
-            per_read = tj.get("dram_bytes_per_read")
-            if per_read:
-                traffic = float(per_read) * len(W3["queries"]) / X.world             # this rank's reads = one byte-pass launch
-                traffic_src = ("static: %s B of DRAM traffic per read from the ncu capture of the 100,000-read launch (profiles/traffic_fill.json, %s) "
-                               "x the reads of one launch; not measured in this run" % (per_read, tj.get("captured", "round 2")))
+        traffic, traffic_src = None, "not measured"
         line = {"metric": METRIC, "value": st3["value"], "unit": "GCUPS", "n_gpus": X.world,
                 "steps": args.steps, "warmup": args.warmup, "ms_per_step": st3["step_ms"], "higher_is_better": True, "scaling": "strong",
                 "vs_baseline": None, "dtype": "s16x2 (byte- and word-score semantics in 16-bit DPX lanes)", "data": "synthetic",
@@ -472,6 +494,8 @@ def main():
                 "phases_ms": {"fill_forward": st3["fill_ms"], "resolve": st3["resolve_ms"], "device_total": st3["device_ms"], "wall": st3["wall_ms"]},
                 "byte_overflows": st3["byte_overflows"], "shards": "cell-balanced contiguous blocks of the read list (ssw_dist.shard_range)"}
         line["parity"] = {"config3": parity_check(W3, got3, args.parity, 1)}
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, "config3", got3)
         if do_cpu:
             sample = args.cpu_sample or 8 * cores
             if not C.have_ref():
@@ -484,7 +508,7 @@ def main():
     subs = {}
     if 2 in only:
         W = C.config_workload(2, **(dict(n_reads=4, **tiny) if X.emu else {}))
-        st, got = run_shape(X, 2, W, max(args.sub_steps, 3), 3, args.e2e_reps)
+        st, got = run_shape(X, 2, W, args.sub_steps, 3, args.e2e_reps)
         if rank0:
             o = sub_result(st, X.world, "config2", "1,000 x 150 bp reads vs 5 Mbp, byte-score path, flag 0 (strong: reads split over the GPUs)")
             ref_len = len(W["refs"][0])
@@ -494,6 +518,8 @@ def main():
             o["roofline"] = {"bound": "hbm", "achieved": alg / fs / 1e9, "peak": hbm_peak, "unit": "GB/s",
                              "frac": alg / fs / 1e9 / hbm_peak, "kernel_ms_per_step": st["fill_ms"]}
             o["parity"] = parity_check(W, got, 64, 1)
+            if args.dump_outputs:
+                dump_outputs(args.dump_outputs, "config2", got)
             if do_cpu:
                 sample = min(len(W["queries"]), 4 * cores)
                 o["cpu_baseline"] = cpu_baseline_obj(W, np.arange(sample), np.zeros(sample), "%d of the 1,000 reads x 5 Mbp" % sample)
@@ -505,6 +531,8 @@ def main():
             o = sub_result(st, X.world, "config4", "protein BLOSUM50, word-score path, flag 0: a %d-query slice of the 10,000 x 300 aa queries x all %d x 400 aa targets "
                            "(queries split over the GPUs, targets replicated; the full grid would return 18 GB of records)" % (args.c4_queries, args.c4_targets))
             o["parity"] = parity_check(W, got, 4096, len(W["refs"]))
+            if args.dump_outputs:
+                dump_outputs(args.dump_outputs, "config4", got)
             if do_cpu:
                 rng = np.random.default_rng(7)
                 k = 4000 * cores
@@ -519,6 +547,8 @@ def main():
                            "CIGARs gathered in two phases: lengths, then payload)")
             o["cigar_words"] = int(len(got[1]))
             o["parity"] = parity_check(W, got, 24, 1)
+            if args.dump_outputs:
+                dump_outputs(args.dump_outputs, "config5", got)
             if do_cpu:
                 sample = min(len(W["queries"]), max(cores, 8))
                 o["cpu_baseline"] = cpu_baseline_obj(W, np.arange(sample), np.zeros(sample), "%d of the 1,000 reads x 100 kbp incl. CIGAR" % sample)

@@ -1,5 +1,5 @@
 /*
- * ssw_common.cuh -- shared device/host definitions of the B200 aligner.
+ * ssw_common.cuh -- shared device/host definitions of the H100 aligner.
  *
  * Terminology (follows the reference, src/ssw.c):
  *   query / read   the profiled sequence (rows of the DP matrix)

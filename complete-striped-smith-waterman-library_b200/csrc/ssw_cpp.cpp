@@ -1,5 +1,5 @@
 /*
- * ssw_cpp.cpp -- StripedSmithWaterman::Aligner over the B200-native libssw.so (include/ssw_cpp.h).
+ * ssw_cpp.cpp -- StripedSmithWaterman::Aligner over the H100-native libssw.so (include/ssw_cpp.h).
  * Behaviour follows the reference's wrapper (src/ssw_cpp.cpp): default tables :18-50, flag derivation :222-229,
  * the result conversion with soft clips :52-88 and the '='/'X' rewrite with the mismatch count :127-220,
  * AlignImpl :334-369, Clear/ReBuild :371-419.  Host-only code; the alignment itself runs on the GPU.

@@ -49,7 +49,7 @@ struct Trace {
 };
 
 /* kernel instance = (lanes per group, rows per lane); rows covered = G*R.  Forward instances favour many rows per
- * lane (fewer shuffles and profile loads per cell; measured on config 2: (8,20) 134 ms, (16,10) 139 ms, (32,5) 178 ms). */
+ * lane (fewer shuffles and profile loads per cell). */
 struct Inst { int G, R; };
 static const Inst kInst[] = {
 	{8, 4}, {8, 5}, {8, 8}, {8, 10}, {8, 16}, {8, 20}, {16, 16}, {16, 20}, {32, 16}, {32, 20},      /* 0..9: forward, by rows */
@@ -76,8 +76,8 @@ struct SswOptions {
 	int grid_arm = -1;              /* "grid_arm": best-cell rows of the device-planned grid are recorded in the last k columns of a reference only
 	                                 * (pairs whose maximum lies earlier are re-done): -1 automatic (protein-like alphabets: padded query
 	                                 * length / 4 + 64, switched off when a pilot group re-does more than 0.2 % of its pairs), 0 off, k > 0 fixed */
-	int64_t latency_cols = (int64_t)5 << 19;   /* "latency_cols": passes over at most this many reference columns (2.6 M: one wave of
-	                                            * 1,024-column items on 148 SMs) use the 32-lane instances */
+	int64_t latency_cols = (int64_t)5 << 19;   /* "latency_cols": passes over at most this many reference columns (2.6 M)
+	                                            * use the 32-lane instances */
 	int force_inst = -1;            /* "inst" (measurements): use this forward instance whenever it covers the query */
 	int tb_maxbw = SSW_TBP_MAXBW;   /* "tb_maxbw": widest band handled by the shared-memory traceback kernel */
 	int tb_spec = -1;               /* "tb_spec": 1 = band-doubling rounds of a task side by side (speculative kernel), 0 = one after the other, -1 = automatic (small batches) */
@@ -821,7 +821,7 @@ static int run_strips(ssw_engine* e, const ssw_batch_params& P, const std::vecto
 				const double rounds = (double)((per + wbest - 1) / wbest);
 				const double waves = ceil((double)(n_same * pp) / (double)e->sm_count);
 				/* a CTA with few warps does not fill an SM: charge it as if it had at least 8 */
-				/* measured: a split CTA needs ~4 % longer per round than an unsplit one (config 5: 29.1 vs 28.0 ms) */
+				/* a split CTA waits on its predecessor's progress word: charge it ~4 % more per round than an unsplit one */
 				const double cost = waves * rounds * (wbest < 8 ? 8.0 / wbest : 1.0) * (pp > 1 ? 1.04 : 1.0);
 				if (cost < best_cost - 1e-9) { best_cost = cost; parts = pp; nw = wbest; }
 			}
@@ -1085,8 +1085,7 @@ static int forward_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Al
 					warm = (int64_t)max_lp + ((int64_t)max_len * S.max_mat + P.gap_extend - 1) / P.gap_extend + 4;
 					warm = (warm + 3) / 4 * 4;
 					/* a launch too small to fill the device (one ssw_align call, the word re-fill of a few overflowed reads) is
-					 * latency-bound: shorter chunks, at the price of more warm-up columns (measured on config 2's re-fill
-					 * launch: 4.07 ms with the 16 x warm-up rule, 3.6 ms with 6 x) */
+					 * latency-bound: shorter chunks, at the price of more warm-up columns */
 					if (e->opt.chunk > 0) chunk = block ? (e->opt.chunk + SSW_CM_BLOCK - 1) / SSW_CM_BLOCK * SSW_CM_BLOCK : e->opt.chunk;
 					else if (latency) chunk = e->opt.small_chunk > 0 ? std::max<int64_t>(e->opt.small_chunk, 2 * warm) : std::max<int64_t>(1024, 2 * warm);   /* a lone call: the device is empty, its duration is one item's sweep */
 					else if (base_chunk < 4096) chunk = e->opt.small_chunk > 0 ? std::max<int64_t>(e->opt.small_chunk, 2 * warm) : std::max<int64_t>(2048, 6 * warm);
@@ -1715,7 +1714,7 @@ static int engine_align_impl(ssw_engine* e, const ssw_batch_params* params,
 	/* Long reads with CIGARs: the banded traceback is a set of long serial chains that leaves most of the device idle, and
 	 * the strip fills before it are throughput-bound.  The batch is cut into slices that run on helper engines (own stream
 	 * and scratch, views of this engine's sequences) from as many host threads, so that one slice's traceback runs under
-	 * the fills of the others (config 5: 329 -> 288 ms with three slices).  A fill CTA takes all registers of an SM, so the
+	 * the fills of the others.  A fill CTA takes all registers of an SM, so the
 	 * overlap is by SMs, not by issue slots: traceback CTAs move in where fill CTAs retire. */
 	{
 		int slices = 1;
@@ -1743,8 +1742,8 @@ static int engine_align_impl(ssw_engine* e, const ssw_batch_params* params,
 			std::vector<int64_t> cut((size_t)slices + 1, 0);
 			{
 				std::vector<double> w((size_t)slices, 1.0);
-				/* automatic: six slices, each 80 % of the one before it (the last slice's traceback is not hidden under any fill;
-				 * config 5: 282 ms with three equal slices, 277 ms like this) */
+				/* automatic: six slices, each 80 % of the one before it (the last slice's traceback is not hidden under any fill,
+				 * so it is the smallest) */
 				const int taper = e->opt.slice_taper > 0 ? e->opt.slice_taper : (auto_slices && slices == 6 ? 80 : 0);
 				if (taper > 0) for (int k = 1; k < slices; ++k) w[k] = w[k - 1] * (double)taper / 100.0;
 				double tot = 0, acc = 0;

@@ -42,7 +42,7 @@
 #define SSW_FILL_WARPS 4
 #define SSW_FILL_THREADS (SSW_FILL_WARPS * 32)
 #ifndef SSW_STRIP_R
-#define SSW_STRIP_R 10                      /* rows per lane of the strip kernel: 320 rows per strip (config 5: R=10 247 ms, 16: 268, 20: 257, 8: 365) */
+#define SSW_STRIP_R 10                      /* rows per lane of the strip kernel: 320 rows per strip */
 #endif
 #define SSW_STRIP_MAXW 16                   /* warps per CTA of the strip kernel */
 #ifndef SSW_FLOOR_PERIOD
@@ -211,15 +211,14 @@ struct SswLaneBest {
  * thread (2Q+1 words: conflict-free 128-bit stores for every Q in use, addresses = one base register + immediates):
  * an event is (R+3)/4 vector stores per half.  With BLOSUM50 and 3/1 gaps, or along the true diagonal of a long read, the
  * running maximum grows with every column and some lane of a warp has an event on almost every step; a snapshot kept in
- * registers made the event 2R register moves (21 % of all executed instructions of the config-4 kernel in round 1,
- * profiles/ncu_fill_cfg4_r1.txt). */
+ * registers makes every event 2R register moves. */
 template <int R, bool SMEM = true>
 struct SswSnap {
 	uint4* base;        /* this thread's slots: (h, q) is base[h * Q + q] */
 	static constexpr int Q = (R + 3) / 4;
 };
-/* Register variant (the strip-pipelined kernel: 10 rows per lane, one CTA per SM whatever its shared memory; measured 3-5 %
- * faster there than the shared-memory snapshot, which needs 127 registers in the split variant). */
+/* Register variant (the strip-pipelined kernel: 10 rows per lane, one CTA per SM whatever its shared memory, so the
+ * snapshot's registers cost no occupancy there). */
 template <int R>
 struct SswSnap<R, false> {
 	uint32_t w[2][R];
@@ -338,7 +337,7 @@ __device__ static __forceinline__ void ssw_reduce_best(const SswLaneBest& lb, in
 /* ---------------------------------------------------------------------------------------------------------- */
 
 #ifndef SSW_FILL_MINB
-#define SSW_FILL_MINB 4                     /* minimum resident CTAs per SM asked of ptxas: 128 registers; 16 warps/SM measured 3 % faster than 12 */
+#define SSW_FILL_MINB 4                     /* minimum resident CTAs per SM asked of ptxas: 128 registers, 16 warps per SM */
 #endif
 /* CM: what the forward pass records of the column maxima (the reference's maxColumn[], ssw.c:338/:540)
  *   0  nothing (reverse pass)
@@ -348,8 +347,8 @@ __device__ static __forceinline__ void ssw_reduce_best(const SswLaneBest& lb, in
  *      re-fills those three blocks per alignment with mode 1.  Chunks start at multiples of SSW_CM_BLOCK. */
 /* WARPS: warps per CTA.  4 by default; 8 where one CTA-shared profile is so large (protein alphabets: 64 KB at 20 rows per
  * lane) that four-warp CTAs would leave the SM with 8 resident warps -- eight warps per profile keep 16. */
-/* ARM: items may carry a late arming position (SswItem.cend, device-planned grids); a template parameter because the extra
- * predicate per step costs the kernels that never use it 1.8 % (measured on config 2). */
+/* ARM: items may carry a late arming position (SswItem.cend, device-planned grids); a template parameter so that the kernels
+ * that never use it do not pay for the extra predicate per step. */
 template <int G, int R, int DIR, int CM, bool TERM, int WARPS = SSW_FILL_WARPS, bool ARM = false>
 __global__ void __launch_bounds__(WARPS * 32, WARPS == SSW_FILL_WARPS ? SSW_FILL_MINB : 2)
 ssw_fill_kernel(const SswItem* __restrict__ items, int n_items,

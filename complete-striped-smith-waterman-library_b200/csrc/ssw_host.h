@@ -92,8 +92,7 @@ inline int ssw_ensure_dyn_smem(const void* fn, size_t smem)
 
 /* Ask for the largest shared-memory carve-out for a kernel, once per (device, kernel).  An SM's L1 / shared-memory split can
  * only change while the SM is idle, so launches whose carve-outs differ do not share an SM: the traceback launches of one
- * round (same kernel, row rings of 16 / 32 / 64 KB per CTA) started up to 18 ms apart (%globaltimer of the tasks, config 5)
- * although all their CTAs would have fitted at once.  With one carve-out for every kernel of the long-read phases (traceback,
+ * round (same kernel, row rings of 16 / 32 / 64 KB per CTA) can start far apart although all their CTAs would fit at once.  With one carve-out for every kernel of the long-read phases (traceback,
  * strip fills) their CTAs go wherever registers and shared memory are free. */
 inline int ssw_prefer_max_smem(const void* fn)
 {

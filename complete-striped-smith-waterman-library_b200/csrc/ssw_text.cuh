@@ -69,8 +69,8 @@ ssw_translate_kernel(SswTextArgs A, const uint8_t* __restrict__ q_text, const in
 /* References delivered as packed codes (SURVEY 8(f) rank 4: the CLI's nucleotide codes are 0..4, main.c:84-93, i.e. 4 bits, or 2 bits
  * for N-free sequences): `packed` is the bit stream of the concatenated references, base i at bits [i*bits, i*bits + bits)
  * (low bits first), unpacked here into the engine's padded 1-byte layout.  The resident layout stays one byte per base on
- * purpose: the fill kernel is bound by the ALU pipe and a per-step nibble extract costs ALU slots (profiles/dpx_peak_r2.json:
- * letter_fetch); the packing halves / quarters what crosses PCIe and what the caller keeps in host memory. */
+ * purpose: the fill kernel is bound by the ALU pipe and a per-step nibble extract costs ALU slots (tools/microbench.cu:
+ * letter fetch); the packing halves / quarters what crosses PCIe and what the caller keeps in host memory. */
 __global__ void __launch_bounds__(256)
 ssw_unpack_kernel(int64_t r_bases, int32_t n_r, int32_t bits, const uint8_t* __restrict__ packed, const int64_t* __restrict__ r_off,
                   const int64_t* __restrict__ r_dst, int8_t* __restrict__ r_codes)

@@ -200,8 +200,8 @@ __device__ static __forceinline__ void ssw_tb_tiles(const bool (&act)[NT], int i
 			if (lane >= d) P[t] = max(P[t], o - d * g);
 		}
 	}
-	/* Shuffles cost this kernel its time (a warp's shuffles do not overlap: measured, a radix-4 scan with 7 independent
-	 * shuffles instead of 5 dependent ones is 35 % slower), so only the ones that are needed are issued:
+	/* Shuffles cost this kernel its time (a warp's shuffles do not overlap, so a radix-4 scan with 7 independent shuffles
+	 * instead of 5 dependent ones is slower), so only the ones that are needed are issued:
 	 *  - df5 needs F of the left neighbour only: F(j) = max(H(j-1) - gapO, F(j-1) - gapE) is what the scan computes
 	 *    (with Y for H and g for gapE: the same value in both gap regimes), hence
 	 *    H(j-1) - gapO > F(j-1) - gapE  <=>  F(j) > F(j-1) - gapE, and H of the neighbour is never fetched;
@@ -682,8 +682,8 @@ static int ssw_traceback_run(cudaStream_t stream, cudaStream_t* side /* 3 side s
 	/* Rounds of band doubling run side by side by the speculative kernel (1: not used).  Narrow bands (up to four tiles per row)
 	 * cost one tile latency per row whatever their width, so all of them go together; of wider ones at most two, so that
 	 * a task that needs only the first loses little. */
-	/* Measured on a B200 (config 5, 1,000 reads of 10 kbp): with a thousand tasks in flight the phase is bound by instruction
-	 * issue, not by the latency of a row, and the speculative rounds make it slower (74 -> 86 ms); a single 10 kbp read
+	/* Config 5 (1,000 reads of 10 kbp): with a thousand tasks in flight the phase is bound by instruction
+	 * issue, not by the latency of a row, and the speculative rounds make it slower; a single 10 kbp read
 	 * (one ssw_align call) is pure latency and gains.  Automatic: on for a handful of tasks only (slices of 250 tasks were
 	 * still slower with it). */
 	const bool spec_on = tb_spec > 0 || (tb_spec < 0 && tasks.size() <= 8);

@@ -1,5 +1,5 @@
 """Host-side Python mirror of the reference's ctypes wrapper (src/ssw_lib.py) on top of
-the B200-native libssw.so, plus the batched interface of include/ssw_batch.h.
+the H100-native libssw.so, plus the batched interface of include/ssw_batch.h.
 
  * ``CSsw`` keeps the reference class's surface (ssw_lib.py:94-197): attributes
    ``ssw_init``, ``init_destroy``, ``ssw_align``, ``align_destroy`` bound with the same

@@ -1,5 +1,5 @@
 /*
- * ssw.h -- C ABI of the B200-native Smith-Waterman aligner (drop-in boundary).
+ * ssw.h -- C ABI of the H100-native Smith-Waterman aligner (drop-in boundary).
  *
  * This header declares the same five entry points, the same result record and
  * the same CIGAR helpers as the SSW library's public header, so that existing
@@ -18,7 +18,7 @@
  *   encoded_ops          <- ssw.h:34      (ssw.c:127-160)
  *   to_cigar_int / cigar_int_to_op / cigar_int_to_len <- ssw.h:171-190
  *
- * The implementation behind these symbols is CUDA (sm_100a); there is no CPU
+ * The implementation behind these symbols is CUDA (sm_90a); there is no CPU
  * compute path.  A call made on a machine without a usable GPU fails loudly
  * (message on stderr, NULL result) instead of falling back.
  *

@@ -1,5 +1,5 @@
 /*
- * ssw_batch.h -- batched C ABI of the B200-native aligner.
+ * ssw_batch.h -- batched C ABI of the H100-native aligner.
  *
  * The reference's API aligns one (query, reference) pair per blocking call
  * (ssw.h:126-134); its CLI loops over reads x references around that call

@@ -1,12 +1,12 @@
 /*
- * ssw_cpp.h -- C++ interface of the B200-native aligner: source-compatible with the reference's
+ * ssw_cpp.h -- C++ interface of the H100-native aligner: source-compatible with the reference's
  * StripedSmithWaterman::Aligner / Filter / Alignment (reference src/ssw_cpp.h:15-62 Alignment and Filter,
  * :64-233 the public members of Aligner), so programs written against the reference's wrapper (its example.cpp)
  * compile unchanged against this header and link libssw_cpp.a + libssw.so.
  *
  * Own text; the private part differs from the reference's (programs must be recompiled, as with any C++ wrapper),
  * and one member is new: AlignBatch(), which sends many queries to the GPU in one call -- a single Align() exposes
- * one (query, reference) pair, far too little work for a B200.
+ * one (query, reference) pair, far too little work for an H100.
  */
 #ifndef SSW_B200_CPP_H
 #define SSW_B200_CPP_H

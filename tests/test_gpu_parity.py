@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box): the CUDA library, called through its C ABI,
+"""GPU parity tests (run on an H100): the CUDA library, called through its C ABI,
 must return bit-identical s_align records to the oracle (and to the unmodified reference
 library oracle/_ref/libssw_ref.so when that prebuilt checker travelled with the snapshot).
 Nothing here reads /root/reference."""
@@ -389,7 +389,7 @@ def test_concurrent_callers(ours, checker, capfd):
         print("\n[concurrent callers] 192 ssw_align calls: one thread %.1f ms, eight threads %.1f ms" % (t_serial * 1e3, t_conc * 1e3))
     # correctness is the assertion; the wall times are evidence (tools/call_bench measures the same from C, without the GIL).
     # Calls this small are bound by host-side driver work, which threads contend for; overlap shows once a call carries
-    # enough device work (profiles/call_latency_r2.md).
+    # enough device work.
     assert t_conc < 4 * t_serial, (t_serial, t_conc)
 
 

@@ -3,12 +3,13 @@
  * against the golden fixtures frozen from the unmodified reference
    (tests/golden/goldens.json -- includes the reference's shipped regression
    golden demo/old.txt, the README sample and the example.c known answer);
- * against the unmodified reference compiled into oracle/_ref/libssw_ref.so on
-   randomised inputs in every parameter regime (skipped where that library is
-   not present);
+ * against the answers of the unmodified reference (compiled into
+   oracle/_ref/libssw_ref.so) to randomised inputs in every parameter regime,
+   frozen in tests/golden/oracle_random_ref.json.gz;
  * formulation 2 (Gotoh + ordered bookkeeping, the GPU spec) against
    formulation 1 (literal striped emulation) in the regime gapO > gapE.
 """
+import gzip
 import json
 import os
 
@@ -98,15 +99,20 @@ def random_case(rng):
                 maskLen=int(rng.choice([5, 15, 20, qlen // 2 + 15])), score_size=int(rng.integers(0, 3)))
 
 
-@pytest.mark.skipif(not C.have_ref(), reason="oracle/_ref/libssw_ref.so not built (reference tree absent)")
+RANDOM_SEED, RANDOM_CASES = 20260924, 2500
+
+
 def test_oracle_matches_reference_random(oracle, capfd):
-    ref = C.load_ref()
-    rng = np.random.default_rng(20260924)
+    """The reference's answers to these cases are frozen in golden/oracle_random_ref.json.gz (golden/make_reference_golden.py)."""
+    with gzip.open(os.path.join(C.GOLDEN, "oracle_random_ref.json.gz"), "rt") as f:
+        expected = json.load(f)
+    assert len(expected) == RANDOM_CASES
+    rng = np.random.default_rng(RANDOM_SEED)
     bad = []
-    for k in range(2500):
+    for k in range(RANDOM_CASES):
         c = random_case(rng)
         a = oracle.align(mark=True, **c)
-        b = ref.align(mark=True, **c)
+        b = expected[k]
         d = C.diff_results(a, b)
         if a and b and (a.get("nm"), a.get("cigar_marked")) != (b.get("nm"), b.get("cigar_marked")):
             d.append(("marked", a.get("cigar_marked"), b.get("cigar_marked")))

@@ -1,4 +1,4 @@
-// tools/microbench.cu -- issue-rate probe for the instructions the fill kernel is made of (B200, sm_100a).
+// tools/microbench.cu -- issue-rate probe for the instructions the fill kernel is made of (H100, sm_90a).
 // For each op: every warp runs ILP independent chains of the op in a long unrolled loop; cycles are read with
 // clock64() around the loop; reported figure = warp-instructions per clock per SM with WARPS resident warps.
 // Output: one JSON object on stdout (kept under profiles/ as dpx_peak.json).
