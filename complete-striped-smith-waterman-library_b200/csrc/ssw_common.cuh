@@ -123,6 +123,8 @@ struct SswAlnDesc {
 	int64_t cm_off;     /* as in SswItem */
 	int32_t scan_all;   /* 1: item records are not column-maximum summaries (strip-pipelined fill): scan every column */
 	int32_t warm;       /* block mode: warm-up columns a re-fill of one block of this pair-task needs */
+	int32_t byte_pad;   /* block mode, byte semantics filled on the word rows: pad rows of the byte padding that the fill left
+	                     * out (the item's lp is the word padding); the resolve re-fills the columns they can change (DESIGN 2) */
 };
 
 /* Output of the resolve kernel (the reference's alignment_end[2], ssw.c:104-108, plus status). */

@@ -55,8 +55,9 @@ static const Inst kInst[] = {
 	{8, 4}, {8, 5}, {8, 8}, {8, 10}, {8, 16}, {8, 20}, {16, 16}, {16, 20}, {32, 16}, {32, 20},      /* 0..9: forward, by rows */
 	{32, 4}, {32, 5}, {32, 8}, {32, 10},                                                            /* 10..13: reverse only (one alignment per warp) */
 	{16, 19},                                                                                       /* 14: forward, 304 rows (300 aa queries in word mode: 5 % fewer rows than (16,20)) */
+	{8, 19},                                                                                        /* 15: forward, 152 rows (150 bp reads on their word rows: 5 % fewer rows than (8,20)) */
 };
-static const int kExtraFwd[] = {14};     /* forward instances outside the 0..9 run (appended so that the "inst" numbers of earlier measurements stay) */
+static const int kExtraFwd[] = {14, 15}; /* forward instances outside the 0..9 run (appended so that the "inst" numbers of earlier measurements stay) */
 static const int kNumFwd = 10;
 static const int kNumInst = (int)(sizeof(kInst) / sizeof(kInst[0]));
 
@@ -129,7 +130,7 @@ struct ssw_engine {
 	/* scratch */
 	SswDevBuf d_items, d_bests, d_alns, d_res, d_colmax, d_tb, d_bnd, d_park, d_emul, d_grid, d_out, d_sync;
 	SswDevBuf d_mark;                                        /* ssw_engine_mark_mismatch: tasks, input CIGARs, marked CIGARs */
-	SswDevBuf d_rf_items, d_rf_bests, d_rf_blk, d_rf_cm;     /* block-maximum mode: re-fill items, their (unused) bests, block ids, column maxima */
+	SswDevBuf d_rf_items, d_rf_bests, d_rf_blk, d_rf_cm;     /* block-maximum mode: re-fill items, their (unused) bests, first columns, column maxima */
 	SswStagedD2H staged;
 	cudaStream_t side[3] = {nullptr, nullptr, nullptr};     /* traceback launches of different kernel shapes run side by side */
 	ssw_engine* kids[SSW_MAX_SLICES] = {};                  /* helper engines of the sliced path (views of this engine's sequences) */
@@ -248,6 +249,7 @@ static int dispatch_fill(ssw_engine* e, int inst, const FillPtrs& fp, int n_item
 	case 12: return launch_fill<32, 8>(e, fp, n_items, dir, cm_mode, share, P);
 	case 13: return launch_fill<32, 10>(e, fp, n_items, dir, cm_mode, share, P);
 	case 14: return launch_fill<16, 19>(e, fp, n_items, dir, cm_mode, share, P);
+	case 15: return launch_fill<8, 19>(e, fp, n_items, dir, cm_mode, share, P);
 	default: break;
 	}
 	return -1;
@@ -312,6 +314,7 @@ static int fill_occupancy(int inst, int n)
 	case 8: occ = fill_occ_of<32, 16>(n); break;
 	case 9: occ = fill_occ_of<32, 20>(n); break;
 	case 14: occ = fill_occ_of<16, 19>(n); break;
+	case 15: occ = fill_occ_of<8, 19>(n); break;
 	default: break;
 	}
 	cache[inst][n] = occ > 0 ? occ : 1;
@@ -675,7 +678,8 @@ static inline bool needs_other(const SswFillResult& r, int word, const Sem& S, b
 }
 
 /* How the column maxima of the fill being resolved are stored (fill kernel CM mode), and -- block mode -- what the
- * re-fill of single blocks needs: the kernel instance of the fill and the scoring parameters. */
+ * re-fill of single blocks needs: a kernel instance that covers the rows of every alignment (those of the fill, or the
+ * byte padding of alignments filled on their word rows: rows >= an item's lp are dead) and the scoring parameters. */
 struct CmMode { int block; int inst; const ssw_batch_params* P; };
 
 /* Launch the resolve kernel(s) over `descs` and fetch the results. */
@@ -690,12 +694,12 @@ static int run_resolve(ssw_engine* e, const std::vector<SswAlnDesc>& descs, bool
 	const int per = SSW_RESOLVE_THREADS / 32;
 	const dim3 grid(((int)descs.size() + per - 1) / per);
 	if (second && cm && cm->block) {
-		/* block maxima: stage 1 (summaries + the three blocks per alignment that need single columns), re-fill of those
-		 * blocks with one word per column, stage 2 */
+		/* block maxima: stage 1 (summaries + the three blocks per alignment that need single columns, and the columns right of
+		 * the mask window of byte alignments filled on their word rows), re-fill of those ranges with one word per column, stage 2 */
 		const size_t n_rf = descs.size() * SSW_REFILL_SLOTS;
 		if (e->d_rf_items.ensure(sizeof(SswItem) * n_rf)) return -1;
 		if (e->d_rf_bests.ensure(sizeof(SswItemBest) * n_rf)) return -1;
-		if (e->d_rf_blk.ensure(sizeof(int32_t) * n_rf)) return -1;
+		if (e->d_rf_blk.ensure(sizeof(int32_t) * n_rf)) return -1;    /* first column of every re-filled range, -1: none */
 		if (e->d_rf_cm.ensure(sizeof(uint32_t) * n_rf * SSW_CM_BLOCK + 64)) return -1;
 		ssw_launch(ssw_resolve_blocks_kernel<0>, grid, dim3(SSW_RESOLVE_THREADS), 0, e->stream, (const SswAlnDesc*)e->d_alns.as<SswAlnDesc>(),
 		           (int)descs.size(), (const SswItemBest*)e->d_bests.as<SswItemBest>(), (const uint32_t*)e->d_colmax.as<uint32_t>(),
@@ -932,9 +936,21 @@ static int forward_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Al
 	int64_t pass_cols = 0;
 	for (size_t i = 0; i < sel.size() && pass_cols <= e->opt.latency_cols; ++i) pass_cols += alns[sel[i]].ref_len;
 	const bool latency = e->opt.force_inst < 0 && pass_cols <= e->opt.latency_cols;
+	/* Byte semantics on the word rows (DESIGN 2): where the byte padding of a read adds pad rows to a word padding that
+	 * already has one (length % 16 in 1..7; 150 bp: 152 rows instead of 160), the extra pad rows only raise column maxima
+	 * to the H of the last word row a few columns earlier.  That changes neither the best cell nor the overflow test, and
+	 * of the second-best scan only the 8 columns right of the mask window, which the block-mode resolve re-fills on the
+	 * byte rows.  So it needs block maxima in every launch of the pass: batch layouts, long references or "cm_block" 1. */
+	bool byte_rows = word == 0 && !latency && e->opt.cm_block != 0 && P.gap_extend > 0 && S.max_mat > 0;
+	if (byte_rows && e->opt.cm_block < 0)
+		for (size_t i = 0; i < sel.size() && byte_rows; ++i) if (alns[sel[i]].ref_len < 32768) byte_rows = false;
+	auto fill_lp = [&](int len) {
+		const int lp = lp_of(len, word);
+		return byte_rows && len % 16 >= 1 && len % 16 <= 7 && pick_inst(lp, -1) >= 0 ? lp_of(len, 1) : lp;
+	};
 	for (size_t i = 0; i < sel.size(); ++i) {
 		const Aln& a = alns[sel[i]];
-		const int lp = lp_of(a.read_len, word);
+		const int lp = fill_lp(a.read_len);
 		int inst = latency ? pick_inst_g32(lp) : -1;
 		if (inst < 0) inst = pick_inst(lp, e->opt.force_inst);
 		(inst < 0 ? long_keys : keys).push_back(Key{inst < 0 ? 0 : inst, a.r, a.q, lp, sel[i]});
@@ -997,7 +1013,7 @@ static int forward_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Al
 		for (const Key& k : keys) if (rank[k.q] < 0) { rank[k.q] = 0; q_inst[k.q] = k.inst; qids.push_back(k.q); }
 		std::sort(qids.begin(), qids.end(), [&](int32_t x, int32_t y) {
 			if (q_inst[x] != q_inst[y]) return q_inst[x] < q_inst[y];
-			const int lx = lp_of((int)(e->q_off[x + 1] - e->q_off[x]), word), ly = lp_of((int)(e->q_off[y + 1] - e->q_off[y]), word);
+			const int lx = fill_lp((int)(e->q_off[x + 1] - e->q_off[x])), ly = fill_lp((int)(e->q_off[y + 1] - e->q_off[y]));
 			return lx != ly ? lx < ly : x < y;
 		});
 		for (size_t i = 0; i < qids.size(); ++i) rank[qids[i]] = (int32_t)i;
@@ -1051,7 +1067,6 @@ static int forward_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Al
 			if (latency) block = false;
 			for (size_t i = k; block && i < pts.size() && pts[i].inst == inst; ++i) if (e->r_len[pts[i].r] < 32768) block = false;
 		}
-		const CmMode cm_mode = {block ? 1 : 0, inst, &P};
 		auto cm_words_of = [&](int32_t ref_len) -> size_t {
 			return block ? ((size_t)ref_len / SSW_CM_BLOCK + 1 + 3) / 4 * 4 : ((size_t)ref_len + 3) / 4 * 4;
 		};
@@ -1136,6 +1151,7 @@ static int forward_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Al
 		std::vector<int64_t> desc_aln;
 		items.reserve((size_t)(share ? padded_items : live_items));
 		int64_t cells = 0;
+		int rf_lp = 0;          /* rows the block re-fill must cover: the byte padding of the alignments filled on their word rows */
 		cm_words = 0;
 		for (size_t i = k; i < k_end; ++i) {
 			const PT& pt = pts[i];
@@ -1145,8 +1161,8 @@ static int forward_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Al
 			const Plan& pl = plan[i - k];
 			SswItem it;
 			memset(&it, 0, sizeof(it));
-			it.qa.off = (int32_t)e->q_off[A.q]; it.qa.len = A.read_len; it.qa.lp = lp_of(A.read_len, word); it.qa.rev = 0;
-			if (B) { it.qb.off = (int32_t)e->q_off[B->q]; it.qb.len = B->read_len; it.qb.lp = lp_of(B->read_len, dual ? 1 : word); it.qb.rev = 0; }
+			it.qa.off = (int32_t)e->q_off[A.q]; it.qa.len = A.read_len; it.qa.lp = fill_lp(A.read_len); it.qa.rev = 0;
+			if (B) { it.qb.off = (int32_t)e->q_off[B->q]; it.qb.len = B->read_len; it.qb.lp = dual ? lp_of(B->read_len, 1) : fill_lp(B->read_len); it.qb.rev = 0; }
 			it.ref_off = e->r_off[pt.r]; it.ref_len = ref_len; it.term_a = -1;
 			if (share && i > k && (pts[i].qa != pts[i - 1].qa || pts[i].qb != pts[i - 1].qb)) {
 				/* the queries change: fill the current CTA with dead items (empty range) of the previous queries */
@@ -1169,6 +1185,8 @@ static int forward_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Al
 				memset(&d, 0, sizeof(d));
 				d.first_item = first_item; d.n_items = pl.n_chunks; d.half = h; d.ref_len = ref_len; d.read_len = X.read_len;
 				d.word = word; d.limit = limit; d.mask_len = X.mask_len; d.cm_off = (int64_t)cm_words; d.warm = pl.warm;
+				d.byte_pad = lp_of(X.read_len, word) - fill_lp(X.read_len);
+				rf_lp = std::max(rf_lp, lp_of(X.read_len, word));
 				if (dual && h == 1) { d.word = 1; d.limit = S.limit_word; }
 				descs.push_back(d);
 				desc_aln.push_back(h ? pt.b : pt.a);
@@ -1181,6 +1199,8 @@ static int forward_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Al
 		tr.lap("forward: fill (copy+kernel)");
 		e->timing.fill_forward_launches += 1;
 		e->timing.cells_forward += cells;
+		const int rows = kInst[inst].G * kInst[inst].R;
+		const CmMode cm_mode = {block ? 1 : 0, rf_lp > rows ? pick_inst(rf_lp, -1) : inst, &P};
 		if (resolve_forward(e, descs, desc_aln, alns, word, S, word_first, refill, &cm_mode, dual)) return -1;
 		tr.lap("forward: resolve");
 		k = k_end;

@@ -53,7 +53,7 @@ ssw_grid_plan_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGridQ*
 	if (live) {
 		SswAlnDesc d;
 		d.first_item = (int32_t)idx; d.n_items = 1; d.half = 0; d.ref_len = it.ref_len; d.read_len = qa.len;
-		d.word = A.word; d.limit = A.limit; d.mask_len = qa.mask_len; d.cm_off = it.cm_off; d.scan_all = 0; d.warm = 0;
+		d.word = A.word; d.limit = A.limit; d.mask_len = qa.mask_len; d.cm_off = it.cm_off; d.scan_all = 0; d.warm = 0; d.byte_pad = 0;
 		const int64_t di = ((int64_t)pi * A.n_r + r) * 2;
 		descs[di] = d;
 		d.half = 1; d.read_len = qb.len; d.mask_len = qb.mask_len;

@@ -123,15 +123,20 @@ ssw_resolve_kernel(const SswAlnDesc* __restrict__ alns, int n_aln,
  * score2/ref2, and emits three re-fill items per alignment (dead ones where nothing is needed): the same pair-task,
  * counted range = one block, warm-up as the chunks of the main launch.  The fill kernel (CM == 1) writes their 64
  * column maxima into a small scratch; stage 2 (ssw_resolve_refill_kernel) folds them in.
+ * A byte alignment filled on its word rows (SswAlnDesc.byte_pad > 0) gets a fourth item: columns [e2, e2 + 8) on the
+ * byte rows, the only allowed columns whose byte column maxima can exceed the word ones in a way the scan sees (DESIGN 2).
+ * Its range starts at e2 rounded down to 4 (the 128-bit column stores of the fill); blocks 0..2 stay on the word rows,
+ * they reproduce the columns the main fill summarised.
  */
-#define SSW_REFILL_SLOTS 3
+#define SSW_REFILL_SLOTS 4
+#define SSW_REFILL_ZONE 3       /* slot of the byte-row columns right of the mask window */
 
 template <int DUMMY = 0>
 __global__ void __launch_bounds__(SSW_RESOLVE_THREADS)
 ssw_resolve_blocks_kernel(const SswAlnDesc* __restrict__ alns, int n_aln,
                           const SswItemBest* __restrict__ bests, const uint32_t* __restrict__ blkmax,
                           const SswItem* __restrict__ items, SswFillResult* __restrict__ out,
-                          SswItem* __restrict__ refill_items, int32_t* __restrict__ refill_blk)
+                          SswItem* __restrict__ refill_items, int32_t* __restrict__ refill_c0)
 {
 	constexpr unsigned FULL = 0xffffffffu;
 	const int lane = threadIdx.x & 31;
@@ -163,10 +168,12 @@ ssw_resolve_blocks_kernel(const SswAlnDesc* __restrict__ alns, int n_aln,
 	if (sc >= d.limit) { r.overflow = d.word ? 2 : 1; if (!d.word) r.score = 255; }
 	else if (unarmed) r.overflow = 3;                 /* the caller re-does the pair with arm 0 */
 
-	int slots[SSW_REFILL_SLOTS] = {-1, -1, -1};
+	int slots[SSW_REFILL_SLOTS] = {-1, -1, -1, -1};     /* block ids; the zone slot: its first column */
+	int zone_end = 0;
 	if (sc > 0 && !r.overflow && d.cm_off != SSW_CM_NONE && d.n_items > 0) {
 		const int e1 = max(pos - d.mask_len, 0);
 		const int e2 = min(pos + d.mask_len, d.ref_len) + (d.word ? 0 : 1);
+		if (d.byte_pad > 0 && e2 < d.ref_len) { slots[SSW_REFILL_ZONE] = e2 & ~3; zone_end = min(e2 + 8, d.ref_len); }
 		const uint32_t* bm = blkmax + d.cm_off;
 		int vx = 0, ix = 0;                  /* best exact candidate: items that do not touch the window */
 		int vb = 0, bb = 0x7fffffff;         /* best fully allowed block of the items that do: (value, smallest block) */
@@ -213,20 +220,25 @@ ssw_resolve_blocks_kernel(const SswAlnDesc* __restrict__ alns, int n_aln,
 		const int64_t slot = (int64_t)idx * SSW_REFILL_SLOTS + lane;
 		SswItem it = items[d.n_items > 0 ? d.first_item : 0];
 		it.term_a = -1; it.cend = 0;
+		int c0 = -1;
 		if (b >= 0) {
-			it.p0 = b * SSW_CM_BLOCK; it.p1 = min(it.p0 + SSW_CM_BLOCK, d.ref_len);
-			it.warm = min(d.warm, it.p0);
+			if (lane == SSW_REFILL_ZONE) {
+				it.p0 = b; it.p1 = zone_end;
+				if (h) it.qb.lp += d.byte_pad; else it.qa.lp += d.byte_pad;
+			} else { it.p0 = b * SSW_CM_BLOCK; it.p1 = min(it.p0 + SSW_CM_BLOCK, d.ref_len); }
+			it.warm = min(d.warm, it.p0);     /* d.warm is taken from the byte padding */
 			it.cm_off = slot * SSW_CM_BLOCK - it.p0;
+			c0 = it.p0;
 		} else { it.p0 = it.p1 = 0; it.warm = 0; it.cm_off = SSW_CM_NONE; }
 		refill_items[slot] = it;
-		refill_blk[slot] = b;
+		refill_c0[slot] = c0;
 	}
 }
 
-/* stage 2: fold the re-filled blocks (single column maxima) into the second-best candidate of stage 1 */
+/* stage 2: fold the re-filled ranges (single column maxima) into the second-best candidate of stage 1 */
 template <int DUMMY = 0>
 __global__ void __launch_bounds__(SSW_RESOLVE_THREADS)
-ssw_resolve_refill_kernel(const SswAlnDesc* __restrict__ alns, int n_aln, const int32_t* __restrict__ refill_blk,
+ssw_resolve_refill_kernel(const SswAlnDesc* __restrict__ alns, int n_aln, const int32_t* __restrict__ refill_c0,
                           const uint32_t* __restrict__ refill_cm, SswFillResult* __restrict__ out)
 {
 	constexpr unsigned FULL = 0xffffffffu;
@@ -243,11 +255,12 @@ ssw_resolve_refill_kernel(const SswAlnDesc* __restrict__ alns, int n_aln, const 
 #pragma unroll
 	for (int s = 0; s < SSW_REFILL_SLOTS; ++s) {
 		const int64_t slot = (int64_t)idx * SSW_REFILL_SLOTS + s;
-		const int b = refill_blk[slot];
-		if (b < 0) continue;
-		for (int j = lane; j < SSW_CM_BLOCK; j += 32) {
-			const int c = b * SSW_CM_BLOCK + j;
-			if (c < d.ref_len && (c < e1 || c >= e2)) {
+		const int c0 = refill_c0[slot];
+		if (c0 < 0) continue;
+		const int c1 = min(s == SSW_REFILL_ZONE ? e2 + 8 : c0 + SSW_CM_BLOCK, d.ref_len);
+		for (int j = lane; c0 + j < c1; j += 32) {
+			const int c = c0 + j;
+			if (c < e1 || c >= e2) {
 				const int v = half_of(refill_cm[slot * SSW_CM_BLOCK + j], h);
 				if (ssw_second_better(v, c, v2, i2)) { v2 = v; i2 = c; }
 			}
