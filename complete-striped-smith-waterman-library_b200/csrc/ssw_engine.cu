@@ -728,11 +728,13 @@ static int run_resolve(ssw_engine* e, const std::vector<SswAlnDesc>& descs, bool
 /*
  * Forward bookkeeping shared by both fill kernels: resolve `descs` (semantics `word`), then, where the result must
  * be replaced by the other semantics (needs_other), either re-resolve on the same column maxima -- possible when
- * both semantics have the same number of pad rows, i.e. the matrices are identical -- or queue the alignment in
- * `refill` for a fill with the other row count.
+ * the rows it was filled on are the padding of the other semantics, i.e. the matrices are identical (the fill never
+ * reads the semantics) -- or queue the alignment in `refill` for a fill with the other row count.
+ * pad_reuse: byte alignments filled on their word rows (byte_pad > 0) count as filled on the word padding.
  */
 static int resolve_forward(ssw_engine* e, std::vector<SswAlnDesc>& descs, const std::vector<int64_t>& desc_aln, std::vector<Aln>& alns,
-                           int word, const Sem& S, bool word_first, std::vector<int64_t>* refill, const CmMode* cm = nullptr, bool dual = false)
+                           int word, const Sem& S, bool word_first, std::vector<int64_t>* refill, const CmMode* cm = nullptr, bool dual = false,
+                           bool pad_reuse = false)
 {
 	std::vector<SswFillResult> res;
 	if (run_resolve(e, descs, true, res, cm)) return -1;
@@ -753,10 +755,13 @@ static int resolve_forward(ssw_engine* e, std::vector<SswAlnDesc>& descs, const 
 		Aln& a = alns[desc_aln[i]];
 		a.fwd = res[i]; a.word = word;
 		if (!needs_other(res[i], word, S, word_first)) continue;
-		if (lp_of(a.read_len, 0) == lp_of(a.read_len, 1)) {
+		/* the rows the alignment was filled on: a byte alignment filled on its word rows (byte_pad > 0, DESIGN 2) is the
+		 * word fill of its read, so its word result lies in the same column maxima and item bests */
+		if (lp_of(a.read_len, word) - (pad_reuse ? descs[i].byte_pad : 0) == lp_of(a.read_len, !word)) {
 			SswAlnDesc d = descs[i];
 			d.word = !word;
 			d.limit = d.word ? S.limit_word : S.limit_byte;
+			d.byte_pad = 0;             /* the byte-row columns right of the mask window matter to byte semantics only */
 			alt.push_back(d);
 			alt_aln.push_back(desc_aln[i]);
 		} else if (refill) refill->push_back(desc_aln[i]);
@@ -1201,7 +1206,13 @@ static int forward_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Al
 		e->timing.cells_forward += cells;
 		const int rows = kInst[inst].G * kInst[inst].R;
 		const CmMode cm_mode = {block ? 1 : 0, rf_lp > rows ? pick_inst(rf_lp, -1) : inst, &P};
-		if (resolve_forward(e, descs, desc_aln, alns, word, S, word_first, refill, &cm_mode, dual)) return -1;
+		/* The word results of byte overflows filled on their word rows are resolved from this launch when it holds every
+		 * pair-task of its kernel instance (the BASELINE shapes: config 3 is one launch per GPU, which then needs no second
+		 * one).  Where the column-maximum budget cuts an instance into several launches, those overflows keep the word
+		 * re-fill after the pass: that multi-launch path keeps the launch structure it had (budget launches + one re-fill),
+		 * and the re-resolve has not been measured there. */
+		const bool split = (k > 0 && pts[k - 1].inst == inst) || (k_end < pts.size() && pts[k_end].inst == inst);
+		if (resolve_forward(e, descs, desc_aln, alns, word, S, word_first, refill, &cm_mode, dual, !split)) return -1;
 		tr.lap("forward: resolve");
 		k = k_end;
 	}
