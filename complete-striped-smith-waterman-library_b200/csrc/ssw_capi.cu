@@ -129,14 +129,9 @@ s_align* ssw_record_from(const ssw_batch_result& r, const uint32_t* pool)
 /* ssw_engine_set_option(NULL, name, value): every engine of the pool, present and future */
 int ssw_default_engines_option(const char* name, int64_t value)
 {
+	/* an unknown option must fail now, even while the pool is empty, not at the first ssw_align */
+	if (!ssw_engine_has_option(name)) { fprintf(stderr, "[libssw-b200] unknown option '%s'\n", name); return -1; }
 	std::lock_guard<std::mutex> lock(g_mu);
-	if (g_pool.empty()) {
-		/* validate the name on a throw-away basis: an unknown option must fail now, not at the first ssw_align */
-		static const char* known[] = {"slices", "slice_taper", "carve", "latency_cols", "parts", "small_chunk", "chunk", "cm_block", "cm_budget_mb", "grid_min", "inst", "super", "tb_maxbw", "tb_spec", "grid_split", "grid_group", "grid_arm"};
-		bool ok = false;
-		for (const char* k : known) if (!strcmp(k, name)) ok = true;
-		if (!ok) { fprintf(stderr, "[libssw-b200] unknown option '%s'\n", name); return -1; }
-	}
 	for (PoolEntry& p : g_pool) if (ssw_engine_set_option(p.e, name, value)) return -1;
 	for (auto& kv : g_pool_options) if (kv.first == name) { kv.second = value; return 0; }
 	g_pool_options.emplace_back(name, value);

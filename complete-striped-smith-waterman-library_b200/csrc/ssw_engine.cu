@@ -20,6 +20,7 @@
 #include <string.h>
 #include <math.h>
 #include <functional>
+#include <utility>
 
 #include "ssw_common.cuh"
 #include "ssw_host.h"
@@ -49,17 +50,31 @@ struct Trace {
 };
 
 /* kernel instance = (lanes per group, rows per lane); rows covered = G*R.  Forward instances favour many rows per
- * lane (fewer shuffles and profile loads per cell). */
-struct Inst { int G, R; };
-static const Inst kInst[] = {
-	{8, 4}, {8, 5}, {8, 8}, {8, 10}, {8, 16}, {8, 20}, {16, 16}, {16, 20}, {32, 16}, {32, 20},      /* 0..9: forward, by rows */
-	{32, 4}, {32, 5}, {32, 8}, {32, 10},                                                            /* 10..13: reverse only (one alignment per warp) */
-	{16, 19},                                                                                       /* 14: forward, 304 rows (300 aa queries in word mode: 5 % fewer rows than (16,20)) */
-	{8, 19},                                                                                        /* 15: forward, 152 rows (150 bp reads on their word rows: 5 % fewer rows than (8,20)) */
+ * lane (fewer shuffles and profile loads per cell).  `fwd`: a candidate of the automatic forward choice (pick_inst).
+ * The index of an instance is its "inst" option value and the number earlier measurements quote: new ones are appended. */
+struct Inst { int G, R; bool fwd; };
+static constexpr Inst kInst[] = {
+	{8, 4, true}, {8, 5, true}, {8, 8, true}, {8, 10, true}, {8, 16, true}, {8, 20, true},        /* 0..9: forward, by rows */
+	{16, 16, true}, {16, 20, true}, {32, 16, true}, {32, 20, true},
+	{32, 4, false}, {32, 5, false}, {32, 8, false}, {32, 10, false},                              /* 10..13: one alignment per warp (reverse pass, latency path) */
+	{16, 19, true},                                                                               /* 14: forward, 304 rows (300 aa queries in word mode: 5 % fewer rows than (16,20)) */
+	{8, 19, true},                                                                                /* 15: forward, 152 rows (150 bp reads on their word rows: 5 % fewer rows than (8,20)) */
 };
-static const int kExtraFwd[] = {14, 15}; /* forward instances outside the 0..9 run (appended so that the "inst" numbers of earlier measurements stay) */
-static const int kNumFwd = 10;
-static const int kNumInst = (int)(sizeof(kInst) / sizeof(kInst[0]));
+static constexpr int kNumInst = (int)(sizeof(kInst) / sizeof(kInst[0]));
+static int inst_rows(int inst) { return kInst[inst].G * kInst[inst].R; }
+
+/* f(InstT<G, R>{}) with the (G, R) of instance `inst`: the one place where a runtime index becomes a kernel instance
+ * (-1: no such instance) */
+template <int G_, int R_> struct InstT { static constexpr int G = G_, R = R_; };
+template <class F, size_t... I>
+static int visit_inst(int inst, F&& f, std::index_sequence<I...>)
+{
+	int rc = -1;
+	(void)((inst == (int)I && (rc = f(InstT<kInst[I].G, kInst[I].R>{}), true)) || ...);
+	return rc;
+}
+template <class F>
+static int visit_inst(int inst, F&& f) { return visit_inst(inst, f, std::make_index_sequence<kNumInst>{}); }
 
 /* Tuning knobs ("ssw_engine_set_option"); every engine has its own copy (helper engines get their parent's). */
 #define SSW_MAX_SLICES 8
@@ -88,22 +103,50 @@ struct SswOptions {
 	int64_t cm_budget = 0;          /* "cm_budget_mb": cap of the column-maximum scratch per launch in bytes (0: half of the free memory; tests) */
 };
 
+/* every option of ssw_engine_set_option with the normalisation of its value (include/ssw_batch.h describes them) */
+struct SswOptionDef { const char* name; void (*set)(SswOptions& o, int64_t v); };
+static const SswOptionDef kOptions[] = {
+	{"slices", [](SswOptions& o, int64_t v) { o.slices = v >= 1 && v <= SSW_MAX_SLICES ? (int)v : 0; }},
+	{"slice_taper", [](SswOptions& o, int64_t v) { o.slice_taper = v >= 1 && v <= 99 ? (int)v : 0; }},
+	{"carve", [](SswOptions& o, int64_t v) { o.carve = v != 0 ? 1 : 0; }},
+	{"latency_cols", [](SswOptions& o, int64_t v) { o.latency_cols = v < 0 ? ((int64_t)5 << 19) : v; }},
+	{"parts", [](SswOptions& o, int64_t v) { o.strip_parts = v == 1 || v == 2 || v == 4 ? (int)v : 0; }},
+	{"small_chunk", [](SswOptions& o, int64_t v) { o.small_chunk = v < 0 ? 0 : (v + 3) / 4 * 4; }},
+	{"chunk", [](SswOptions& o, int64_t v) { o.chunk = v < 0 ? 0 : (v + 3) / 4 * 4; }},
+	{"cm_block", [](SswOptions& o, int64_t v) { o.cm_block = v < 0 ? -1 : (v ? 1 : 0); }},
+	{"cm_budget_mb", [](SswOptions& o, int64_t v) { o.cm_budget = v <= 0 ? 0 : v << 20; }},
+	{"grid_split", [](SswOptions& o, int64_t v) { o.grid_split_pairs = v < 0 ? (int64_t)4 << 20 : v; }},
+	{"grid_arm", [](SswOptions& o, int64_t v) { o.grid_arm = v < 0 ? -1 : (int)v; }},
+	{"grid_group", [](SswOptions& o, int64_t v) { o.grid_group_qp = v < 1 ? 16 : (int)v; }},
+	{"grid_min", [](SswOptions& o, int64_t v) { o.grid_min_pairs = v < 0 ? 32768 : (int)v; }},
+	{"inst", [](SswOptions& o, int64_t v) { o.force_inst = (int)v; }},       /* index into kInst */
+	{"super", [](SswOptions& o, int64_t v) { o.strip_super = v >= 64 ? (int)(v + 7) / 8 * 8 : SSW_STRIP_SUPER; }},
+	{"tb_spec", [](SswOptions& o, int64_t v) { o.tb_spec = v < 0 ? -1 : (int)v; }},      /* > 1: on, rounds up to that many columns */
+	{"tb_maxbw", [](SswOptions& o, int64_t v) { o.tb_maxbw = v < 0 ? SSW_TBP_MAXBW : (int)std::min<int64_t>(v, SSW_TBP_MAXBW); }},
+};
+static const SswOptionDef* find_option(const char* name)
+{
+	for (const SswOptionDef& d : kOptions) if (!strcmp(d.name, name)) return &d;
+	return nullptr;
+}
+
+/* the forward (g32 false) or 32-lane (g32 true) instance with the fewest rows >= lp; -1: none covers lp */
+static int fewest_rows(int lp, bool g32)
+{
+	int best = -1, best_rows = 0;
+	for (int i = 0; i < kNumInst; ++i) {
+		const int rows = inst_rows(i);
+		if ((g32 ? kInst[i].G == 32 : kInst[i].fwd) && rows >= lp && (best < 0 || rows < best_rows)) { best = i; best_rows = rows; }
+	}
+	return best;
+}
 static int pick_inst(int lp, int force_inst)
 {
-	if (force_inst >= 0 && force_inst < kNumInst && kInst[force_inst].G * kInst[force_inst].R >= lp) return force_inst;   /* 10..13: the 32-lane layouts */
-	int best = -1;
-	for (int i = 0; i < kNumFwd; ++i) if (kInst[i].G * kInst[i].R >= lp) { best = i; break; }
-	for (int i : kExtraFwd) if (kInst[i].G * kInst[i].R >= lp && (best < 0 || kInst[i].G * kInst[i].R < kInst[best].G * kInst[best].R)) best = i;
-	if (best >= 0) return best;
-	return -1;
+	if (force_inst >= 0 && force_inst < kNumInst && inst_rows(force_inst) >= lp) return force_inst;   /* any instance, 10..13 included */
+	return fewest_rows(lp, false);
 }
 /* reverse pass: one alignment per warp */
-static int pick_inst_g32(int lp)
-{
-	static const int order[] = {10, 11, 12, 13, 8, 9};
-	for (int i : order) if (kInst[i].G * kInst[i].R >= lp) return i;
-	return -1;
-}
+static int pick_inst_g32(int lp) { return fewest_rows(lp, true); }
 
 }  // namespace
 
@@ -162,97 +205,67 @@ struct ssw_engine {
 
 struct FillPtrs { const SswItem* items; uint32_t* cm; SswItemBest* bests; bool arm = false; /* items carry late arming positions (grid path) */ };
 
-/* Warps per CTA of a forward launch with a CTA-shared profile: 8 instead of 4 when that doubles the resident warps per SM
- * (large alphabets: the profile, not the registers, limits the CTAs per SM). */
+/* Warps per CTA and dynamic shared memory of a fill launch with R rows per lane for an alphabet of n letters.  Per-warp
+ * profiles (share == 0) can be large for big alphabets: fewer warps per CTA then.  A forward launch with a CTA-shared
+ * profile takes 8 warps instead of 4 when that doubles the resident warps per SM (large alphabets: the profile, not the
+ * registers, limits the CTAs per SM). */
+struct FillShape { int warps; size_t smem; };
 template <int R>
-static int fill_warps_shared(int n)
+static FillShape fill_shape(int n, int share, int dir)
 {
-	if (R < 16) return SSW_FILL_WARPS;
-	const size_t prof = ssw_fill_smem_bytes<R>(n, 1), snap = ssw_snap_smem_bytes<R>(32), sm = (size_t)227 * 1024;
-	const size_t s4 = prof + snap * 4 + 1024, s8 = prof + snap * 8 + 1024;
-	const int occ4 = (int)std::min<size_t>(SSW_FILL_MINB, sm / s4), occ8 = (int)std::min<size_t>(2, sm / s8);
-	return occ8 * 8 > occ4 * 4 ? 8 : SSW_FILL_WARPS;
-}
-static int fill_warps_of(int inst, int n, int share)
-{
-	if (!share) return SSW_FILL_WARPS;
-	switch (kInst[inst].R) {
-	case 16: return fill_warps_shared<16>(n);
-	case 19: return fill_warps_shared<19>(n);
-	case 20: return fill_warps_shared<20>(n);
-	default: return SSW_FILL_WARPS;
+	const size_t prof = ssw_fill_smem_bytes<R>(n, 1), snap = ssw_snap_smem_bytes<R>(32);
+	int warps = SSW_FILL_WARPS;
+	if (!share) while (warps > 1 && (prof + snap) * warps > 200 * 1024) --warps;
+	else if (dir > 0 && R >= 16) {
+		const size_t sm = (size_t)227 * 1024, s4 = prof + snap * 4 + 1024, s8 = prof + snap * 8 + 1024;
+		const int occ4 = (int)std::min<size_t>(SSW_FILL_MINB, sm / s4), occ8 = (int)std::min<size_t>(2, sm / s8);
+		if (occ8 * 8 > occ4 * 4) warps = 8;
 	}
+	return FillShape{warps, (share ? prof : prof * warps) + snap * warps};       /* profile(s), then the best-cell snapshots */
+}
+
+/* items per CTA of a forward launch of instance `inst` with CTA-shared profiles */
+static int fill_items_per_cta(int inst, int n)
+{
+	return visit_inst(inst, [n](auto t) { using T = decltype(t); return fill_shape<T::R>(n, 1, +1).warps * (32 / T::G); });
 }
 
 template <int G, int R>
 static int launch_fill(ssw_engine* e, const FillPtrs& fp, int n_items, int dir, int cm_mode, int share, const ssw_batch_params& P)
 {
-	constexpr int GPW = 32 / G;
-	/* per-warp profiles (share == 0) can be large for big alphabets: use fewer warps per CTA then */
-	const size_t warp_smem = ssw_fill_smem_bytes<R>(P.n, 1), warp_snap = ssw_snap_smem_bytes<R>(32);
-	int warps = SSW_FILL_WARPS;
-	if (!share) while (warps > 1 && (warp_smem + warp_snap) * warps > 200 * 1024) --warps;
-	else if (dir > 0) warps = fill_warps_shared<R>(P.n);
-	const int per_cta = warps * GPW;
+	const FillShape sh = fill_shape<R>(P.n, share, dir);
+	if (sh.smem > 220 * 1024) { fprintf(stderr, "[libssw-b200] alphabet of %d letters is too large for this query length\n", P.n); return -2; }
+	const int per_cta = sh.warps * (32 / G);
 	const int grid = (n_items + per_cta - 1) / per_cta;
-	const size_t smem = (share ? warp_smem : warp_smem * warps) + warp_snap * warps;       /* profile(s), then the best-cell snapshots */
-	if (smem > 220 * 1024) { fprintf(stderr, "[libssw-b200] alphabet of %d letters is too large for this query length\n", P.n); return -2; }
-	const SswItem* items = fp.items;
 	const int8_t* q = e->d_q.as<int8_t>();
 	const int8_t* r = e->d_r.as<int8_t>();
 	const int8_t* mat = e->d_mat.as<int8_t>();
-	uint32_t* cm = fp.cm;
-	SswItemBest* bests = fp.bests;
-#define SSW_FILL_GO(DIR, CM, TERM, W, ARM)                                                                       \
-	do {                                                                                                         \
-		auto kern = ssw_fill_kernel<G, R, DIR, CM, TERM, W, ARM>;                                                \
-		if (ssw_ensure_dyn_smem(reinterpret_cast<const void*>(kern), smem)) return -1;                           \
-		ssw_launch(kern, dim3(grid), dim3(warps * 32), smem, e->stream, items, n_items, q, r, mat, (int)P.n,     \
-		           (int)P.gap_open, (int)P.gap_extend, cm, bests, share);                                        \
-	} while (0)
-	if (dir > 0) {   /* forward: column maxima per column or per block */
-		if (warps == 8) {
-			if constexpr (R >= 16) {
-				if (cm_mode == 2) SSW_FILL_GO(1, 2, false, 8, false);
-				else if (fp.arm) SSW_FILL_GO(1, 1, false, 8, true);
-				else SSW_FILL_GO(1, 1, false, 8, false);
-			}
-			else return -2;
-		}
-		else if (cm_mode == 2) SSW_FILL_GO(1, 2, false, SSW_FILL_WARPS, false);
-		else if (fp.arm) SSW_FILL_GO(1, 1, false, SSW_FILL_WARPS, true);
-		else SSW_FILL_GO(1, 1, false, SSW_FILL_WARPS, false);
-	} else {
-		if constexpr (G == 32) SSW_FILL_GO(-1, 0, true, SSW_FILL_WARPS, false);   /* reverse: one alignment per warp, early termination */
-		else return -2;
+	auto go = [&](auto kern) {
+		if (ssw_ensure_dyn_smem(reinterpret_cast<const void*>(kern), sh.smem)) return -1;
+		ssw_launch(kern, dim3(grid), dim3(sh.warps * 32), sh.smem, e->stream, fp.items, n_items, q, r, mat, (int)P.n,
+		           (int)P.gap_open, (int)P.gap_extend, fp.cm, fp.bests, share);
+		SSW_CUDA_OK(cudaGetLastError());
+		return 0;
+	};
+	if (dir < 0) {   /* reverse: one alignment per warp, early termination */
+		if constexpr (G == 32) return go(ssw_fill_kernel<G, R, -1, 0, true, SSW_FILL_WARPS, false>);
+		return -2;
 	}
-#undef SSW_FILL_GO
-	SSW_CUDA_OK(cudaGetLastError());
-	return 0;
+	/* forward: column maxima per column or per block */
+	if (sh.warps == 8) {
+		if constexpr (R >= 16) {
+			if (cm_mode == 2) return go(ssw_fill_kernel<G, R, 1, 2, false, 8, false>);
+			return fp.arm ? go(ssw_fill_kernel<G, R, 1, 1, false, 8, true>) : go(ssw_fill_kernel<G, R, 1, 1, false, 8, false>);
+		}
+		return -2;
+	}
+	if (cm_mode == 2) return go(ssw_fill_kernel<G, R, 1, 2, false, SSW_FILL_WARPS, false>);
+	return fp.arm ? go(ssw_fill_kernel<G, R, 1, 1, false, SSW_FILL_WARPS, true>) : go(ssw_fill_kernel<G, R, 1, 1, false, SSW_FILL_WARPS, false>);
 }
 
 static int dispatch_fill(ssw_engine* e, int inst, const FillPtrs& fp, int n_items, int dir, int cm_mode, int share, const ssw_batch_params& P)
 {
-	switch (inst) {
-	case 0: return launch_fill<8, 4>(e, fp, n_items, dir, cm_mode, share, P);
-	case 1: return launch_fill<8, 5>(e, fp, n_items, dir, cm_mode, share, P);
-	case 2: return launch_fill<8, 8>(e, fp, n_items, dir, cm_mode, share, P);
-	case 3: return launch_fill<8, 10>(e, fp, n_items, dir, cm_mode, share, P);
-	case 4: return launch_fill<8, 16>(e, fp, n_items, dir, cm_mode, share, P);
-	case 5: return launch_fill<8, 20>(e, fp, n_items, dir, cm_mode, share, P);
-	case 6: return launch_fill<16, 16>(e, fp, n_items, dir, cm_mode, share, P);
-	case 7: return launch_fill<16, 20>(e, fp, n_items, dir, cm_mode, share, P);
-	case 8: return launch_fill<32, 16>(e, fp, n_items, dir, cm_mode, share, P);
-	case 9: return launch_fill<32, 20>(e, fp, n_items, dir, cm_mode, share, P);
-	case 10: return launch_fill<32, 4>(e, fp, n_items, dir, cm_mode, share, P);      /* 10..13: the 32-lane layouts (reverse pass, latency path, "inst" option) */
-	case 11: return launch_fill<32, 5>(e, fp, n_items, dir, cm_mode, share, P);
-	case 12: return launch_fill<32, 8>(e, fp, n_items, dir, cm_mode, share, P);
-	case 13: return launch_fill<32, 10>(e, fp, n_items, dir, cm_mode, share, P);
-	case 14: return launch_fill<16, 19>(e, fp, n_items, dir, cm_mode, share, P);
-	case 15: return launch_fill<8, 19>(e, fp, n_items, dir, cm_mode, share, P);
-	default: break;
-	}
-	return -1;
+	return visit_inst(inst, [&](auto t) { using T = decltype(t); return launch_fill<T::G, T::R>(e, fp, n_items, dir, cm_mode, share, P); });
 }
 
 int ssw_engine::run_fill(const std::vector<SswItem>& items, int inst, int dir, int cm_mode, int share, const ssw_batch_params& P, float* ms_acc)
@@ -275,50 +288,24 @@ int ssw_engine::run_fill(const std::vector<SswItem>& items, int inst, int dir, i
 
 
 /* resident CTAs per SM of the forward fill kernel of instance `inst` in CTA-shared-profile mode */
-template <int G, int R>
-static int fill_occ_of(int n)
-{
-	int occ = 0;
-	const int warps = fill_warps_shared<R>(n);
-	const size_t smem = ssw_fill_smem_bytes<R>(n, 1) + ssw_snap_smem_bytes<R>(warps * 32);
-	if (warps == 8) {
-		if constexpr (R >= 16) {
-			auto kern = ssw_fill_kernel<G, R, 1, 2, false, 8>;
-			ssw_ensure_dyn_smem(reinterpret_cast<const void*>(kern), smem);
-			if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, 256, smem) != cudaSuccess) occ = 1;
-		}
-		return occ > 0 ? occ : 1;
-	}
-	auto kern = ssw_fill_kernel<G, R, 1, 2, false>;
-	ssw_ensure_dyn_smem(reinterpret_cast<const void*>(kern), smem);
-	if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, SSW_FILL_THREADS, smem) != cudaSuccess) occ = 1;
-	return occ;
-}
 static int fill_occupancy(int inst, int n)
 {
-	static int cache[16][65];
+	static int cache[kNumInst][65];
 	static std::mutex mu;
-	if (inst < 0 || inst >= 16 || n < 0 || n > 64) return 1;
+	if (inst < 0 || inst >= kNumInst || n < 0 || n > 64) return 1;
 	std::lock_guard<std::mutex> lock(mu);
-	if (cache[inst][n]) return cache[inst][n];
-	int occ = 1;
-	switch (inst) {
-	case 0: occ = fill_occ_of<8, 4>(n); break;
-	case 1: occ = fill_occ_of<8, 5>(n); break;
-	case 2: occ = fill_occ_of<8, 8>(n); break;
-	case 3: occ = fill_occ_of<8, 10>(n); break;
-	case 4: occ = fill_occ_of<8, 16>(n); break;
-	case 5: occ = fill_occ_of<8, 20>(n); break;
-	case 6: occ = fill_occ_of<16, 16>(n); break;
-	case 7: occ = fill_occ_of<16, 20>(n); break;
-	case 8: occ = fill_occ_of<32, 16>(n); break;
-	case 9: occ = fill_occ_of<32, 20>(n); break;
-	case 14: occ = fill_occ_of<16, 19>(n); break;
-	case 15: occ = fill_occ_of<8, 19>(n); break;
-	default: break;
-	}
-	cache[inst][n] = occ > 0 ? occ : 1;
-	return cache[inst][n];
+	int& occ = cache[inst][n];
+	if (!occ) occ = std::max(1, visit_inst(inst, [n](auto t) {
+		using T = decltype(t);
+		const FillShape sh = fill_shape<T::R>(n, 1, +1);
+		auto kern = ssw_fill_kernel<T::G, T::R, 1, 2, false, SSW_FILL_WARPS, false>;
+		if constexpr (T::R >= 16) if (sh.warps == 8) kern = ssw_fill_kernel<T::G, T::R, 1, 2, false, 8, false>;
+		ssw_ensure_dyn_smem(reinterpret_cast<const void*>(kern), sh.smem);
+		int blocks = 0;
+		if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, kern, sh.warps * 32, sh.smem) != cudaSuccess) blocks = 1;
+		return blocks;
+	}));
+	return occ;
 }
 
 /* ------------------------------------------------------------------------------------------- */
@@ -374,27 +361,13 @@ extern "C" int ssw_engine_set_option(ssw_engine* e, const char* name, int64_t va
 {
 	if (!name) return -1;
 	if (!e) return ssw_default_engines_option(name, value);
-	SswOptions& o = e->opt;
-	if (!strcmp(name, "slices")) { o.slices = value >= 1 && value <= SSW_MAX_SLICES ? (int)value : 0; return 0; }
-	if (!strcmp(name, "slice_taper")) { o.slice_taper = value >= 1 && value <= 99 ? (int)value : 0; return 0; }
-	if (!strcmp(name, "carve")) { o.carve = value != 0 ? 1 : 0; return 0; }
-	if (!strcmp(name, "latency_cols")) { o.latency_cols = value < 0 ? ((int64_t)5 << 19) : value; return 0; }
-	if (!strcmp(name, "parts")) { o.strip_parts = value == 1 || value == 2 || value == 4 ? (int)value : 0; return 0; }
-	if (!strcmp(name, "small_chunk")) { o.small_chunk = value < 0 ? 0 : (value + 3) / 4 * 4; return 0; }
-	if (!strcmp(name, "chunk")) { o.chunk = value < 0 ? 0 : (value + 3) / 4 * 4; return 0; }
-	if (!strcmp(name, "cm_block")) { o.cm_block = value < 0 ? -1 : (value ? 1 : 0); return 0; }
-	if (!strcmp(name, "cm_budget_mb")) { o.cm_budget = value <= 0 ? 0 : value << 20; return 0; }
-	if (!strcmp(name, "grid_split")) { o.grid_split_pairs = value < 0 ? (int64_t)4 << 20 : value; return 0; }
-	if (!strcmp(name, "grid_arm")) { o.grid_arm = value < 0 ? -1 : (int)value; return 0; }
-	if (!strcmp(name, "grid_group")) { o.grid_group_qp = value < 1 ? 16 : (int)value; return 0; }
-	if (!strcmp(name, "grid_min")) { o.grid_min_pairs = value < 0 ? 32768 : (int)value; return 0; }
-	if (!strcmp(name, "inst")) { o.force_inst = (int)value; return 0; }       /* index into kInst */
-	if (!strcmp(name, "super")) { o.strip_super = value >= 64 ? (int)(value + 7) / 8 * 8 : SSW_STRIP_SUPER; return 0; }
-	if (!strcmp(name, "tb_spec")) { o.tb_spec = value < 0 ? -1 : (int)value; return 0; }      /* > 1: on, rounds up to that many columns */
-	if (!strcmp(name, "tb_maxbw")) { o.tb_maxbw = value < 0 ? SSW_TBP_MAXBW : (int)std::min<int64_t>(value, SSW_TBP_MAXBW); return 0; }
-	fprintf(stderr, "[libssw-b200] unknown option '%s'\n", name);
-	return -1;
+	const SswOptionDef* d = find_option(name);
+	if (!d) { fprintf(stderr, "[libssw-b200] unknown option '%s'\n", name); return -1; }
+	d->set(e->opt, value);
+	return 0;
 }
+
+bool ssw_engine_has_option(const char* name) { return find_option(name) != nullptr; }
 
 extern "C" int ssw_engine_last_timing(const ssw_engine* e, ssw_engine_timing* t)
 {
@@ -403,7 +376,22 @@ extern "C" int ssw_engine_last_timing(const ssw_engine* e, ssw_engine_timing* t)
 	return 0;
 }
 
-/* references are stored as  [PAD x null] codes [PAD x null]  with null = n (scores as a dead letter) */
+/* References are stored as  [PAD x null] codes [PAD x null]  with null = n (scores as a dead letter), each block
+ * 16-aligned; the fill kernels rely on those pads (col_lo / col_hi in ssw_fill.cuh).  Fills r_off with the offset of
+ * column 0 of every reference and returns the length of the padded array. */
+static int64_t ref_layout(const std::vector<int32_t>& r_len, std::vector<int64_t>& r_off)
+{
+	int64_t total = 0;
+	r_off.resize(r_len.size());
+	for (size_t i = 0; i < r_len.size(); ++i) {
+		total += SSW_REF_PAD;
+		r_off[i] = total;
+		total += (int64_t)r_len[i] + SSW_REF_PAD;
+		total = (total + 15) / 16 * 16;
+	}
+	return total + 2 * SSW_REF_PAD;
+}
+
 int ssw_engine::upload_refs(int n)
 {
 	if (padded_n == n && d_r.p) return 0;
@@ -411,16 +399,7 @@ int ssw_engine::upload_refs(int n)
 		fprintf(stderr, "[libssw-b200] sequences were set as text for an alphabet of %d letters; this call uses %d\n", padded_n, n);
 		return -1;
 	}
-	int64_t total = 0;
-	r_off.resize(n_r);
-	for (int i = 0; i < n_r; ++i) {
-		total += SSW_REF_PAD;
-		r_off[i] = total;
-		total += r_len[i];
-		total += SSW_REF_PAD;
-		total = (total + 15) / 16 * 16;
-	}
-	total += 2 * SSW_REF_PAD;
+	const int64_t total = ref_layout(r_len, r_off);
 	std::vector<int8_t> padded((size_t)total, (int8_t)n);
 	for (int i = 0; i < n_r; ++i) memcpy(padded.data() + r_off[i], h_r.data() + h_r_off[i], (size_t)r_len[i]);
 	if (d_r.ensure((size_t)total)) return -1;
@@ -525,17 +504,8 @@ static int set_sequences_packed_impl(ssw_engine* e, int32_t n_queries, const int
 	e->h_q.assign(queries, queries + qb);
 	e->h_r.clear(); e->h_r_off.clear();
 	e->r_len.resize(n_refs);
-	e->r_off.resize(n_refs);
-	int64_t total = 0;
-	for (int i = 0; i < n_refs; ++i) {
-		e->r_len[i] = (int32_t)(ref_off[i + 1] - ref_off[i]);
-		total += SSW_REF_PAD;
-		e->r_off[i] = total;
-		total += e->r_len[i];
-		total += SSW_REF_PAD;
-		total = (total + 15) / 16 * 16;
-	}
-	total += 2 * SSW_REF_PAD;
+	for (int i = 0; i < n_refs; ++i) e->r_len[i] = (int32_t)(ref_off[i + 1] - ref_off[i]);
+	const int64_t total = ref_layout(e->r_len, e->r_off);
 	const size_t pk = (size_t)((rb * bits + 7) / 8);
 	const size_t o_ro = (pk + 255) / 256 * 256, o_rd = o_ro + 8 * (size_t)(n_refs + 1);
 	if (e->d_grid.ensure(o_rd + 8 * (size_t)(n_refs + 1) + 256)) return -1;
@@ -600,17 +570,8 @@ static int set_sequences_text_impl(ssw_engine* e,
 	if (rc) for (int i = 1; i <= n_queries; ++i) e->q_off.push_back(qb + query_off[i]);
 	e->h_q.clear(); e->h_r.clear(); e->h_r_off.clear();
 	e->r_len.resize(n_refs);
-	e->r_off.resize(n_refs);
-	int64_t total = 0;
-	for (int i = 0; i < n_refs; ++i) {
-		e->r_len[i] = (int32_t)(ref_off[i + 1] - ref_off[i]);
-		total += SSW_REF_PAD;
-		e->r_off[i] = total;
-		total += e->r_len[i];
-		total += SSW_REF_PAD;
-		total = (total + 15) / 16 * 16;
-	}
-	total += 2 * SSW_REF_PAD;
+	for (int i = 0; i < n_refs; ++i) e->r_len[i] = (int32_t)(ref_off[i + 1] - ref_off[i]);
+	const int64_t total = ref_layout(e->r_len, e->r_off);
 	/* staging: texts, offsets, destination offsets, table */
 	const size_t o_qt = 0, o_rt = (size_t)(qb + 255) / 256 * 256, o_qo = o_rt + (size_t)(rb + 255) / 256 * 256;
 	const size_t o_ro = o_qo + 8 * (size_t)(n_queries + 1), o_rd = o_ro + 8 * (size_t)(n_refs + 1), o_tab = o_rd + 8 * (size_t)(n_refs + 1);
@@ -1061,7 +1022,7 @@ static int forward_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Al
 	while (k < pts.size()) {
 		/* one launch = one kernel instance, bounded by the column-maximum budget */
 		const int inst = pts[k].inst;
-		const int per_cta = fill_warps_of(inst, P.n, 1) * (32 / kInst[inst].G);   /* items per CTA of a launch with CTA-shared profiles */
+		const int per_cta = fill_items_per_cta(inst, P.n);   /* items per CTA of a launch with CTA-shared profiles */
 		size_t k_end = k, cm_words = 0;
 		int64_t total_cols = 0;
 		/* Column maxima: one word per column, or -- long references in a launch that fills the device -- one word per block of
@@ -1182,7 +1143,7 @@ static int forward_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Al
 				it.warm = std::min(pl.warm, it.p0);
 				it.cm_off = (int64_t)cm_words;
 				items.push_back(it);
-				cells += (int64_t)(it.p1 - it.p0 + it.warm) * kInst[inst].G * kInst[inst].R * 2;
+				cells += (int64_t)(it.p1 - it.p0 + it.warm) * inst_rows(inst) * 2;
 			}
 			for (int h = 0; h < (B ? 2 : 1); ++h) {
 				const Aln& X = h ? *B : A;
@@ -1204,7 +1165,7 @@ static int forward_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Al
 		tr.lap("forward: fill (copy+kernel)");
 		e->timing.fill_forward_launches += 1;
 		e->timing.cells_forward += cells;
-		const int rows = kInst[inst].G * kInst[inst].R;
+		const int rows = inst_rows(inst);
 		const CmMode cm_mode = {block ? 1 : 0, rf_lp > rows ? pick_inst(rf_lp, -1) : inst, &P};
 		/* The word results of byte overflows filled on their word rows are resolved from this launch when it holds every
 		 * pair-task of its kernel instance (the BASELINE shapes: config 3 is one launch per GPU, which then needs no second
@@ -1431,7 +1392,7 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 	size_t k = 0;
 	while (k < order.size()) {
 		const int inst = q_inst[order[k]];
-		const int per_cta = fill_warps_of(inst, P.n, 1) * (32 / kInst[inst].G);
+		const int per_cta = fill_items_per_cta(inst, P.n);
 		const int n_r_pad = (n_r + per_cta - 1) / per_cta * per_cta;
 		/* query pairs of this launch: same instance, bounded by memory */
 		const size_t per_qp = (size_t)cm_per_qp * 4 + (size_t)n_r_pad * (sizeof(SswItem) + sizeof(SswItemBest)) + (size_t)n_r * 2 * (sizeof(SswAlnDesc) + sizeof(SswFillResult));
@@ -1482,7 +1443,7 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 			if (rc) return rc < 0 ? rc : -1;
 			e->laps.stop(e->stream, &e->timing.fill_forward_ms);
 			e->timing.fill_forward_launches += 1;
-			e->timing.cells_forward += (int64_t)A.n_qp * (cm_per_qp) * kInst[inst].G * kInst[inst].R * 2;
+			e->timing.cells_forward += (int64_t)A.n_qp * (cm_per_qp) * inst_rows(inst) * 2;
 		}
 		e->laps.start(e->stream);
 		{

@@ -188,6 +188,7 @@ struct SswStagedD2H {
 struct ssw_engine;
 extern "C" int ssw_engine_set_pair(ssw_engine* e, const int8_t* read, int32_t readLen, const int8_t* ref, int32_t refLen);
 int ssw_default_engines_option(const char* name, int64_t value);     /* ssw_engine_set_option(NULL, ...): the engines behind ssw_align */
+bool ssw_engine_has_option(const char* name);                        /* is `name` an option of ssw_engine_set_option */
 
 /* Phase times without synchronising: start/stop only record events on the stream; the elapsed times are read and added
  * to their accumulators by collect(), once, after the call's final synchronisation.  (A stopwatch that waits for its stop
