@@ -56,13 +56,16 @@ def fill_rows(read, ref, mat, n, gap_o, gap_e, lp):
     return out
 
 
-def spill_identity_holds(read, ref, mat, n, gap_o, gap_e):
+def spill_identity_holds(read, ref, mat, n, gap_o, gap_e, spill_cols=None):
+    """spill_cols: how many earlier columns of the last word row spill into a byte column maximum (default: one per extra
+    byte pad row, as DESIGN 2 proves; fewer must break the identity)"""
     L = len(read)
     lw, lb = lp_of(L, 1), lp_of(L, 0)
     H = fill_rows(read, ref, mat, n, gap_o, gap_e, lb)
     cw, cb = H[:lw].max(axis=0), H.max(axis=0)
     h = np.concatenate((np.zeros(lb - lw, dtype=np.int64), H[lw - 1]))
-    spill = np.max([h[lb - lw - k: lb - lw - k + len(ref)] for k in range(1, lb - lw + 1)], axis=0)
+    ks = range(1, (lb - lw if spill_cols is None else spill_cols) + 1)
+    spill = np.max([h[lb - lw - k: lb - lw - k + len(ref)] for k in ks], axis=0)
     return np.array_equal(cb, np.maximum(cw, spill))
 
 
