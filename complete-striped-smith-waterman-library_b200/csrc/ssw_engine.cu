@@ -172,6 +172,7 @@ struct ssw_engine {
 
 	/* scratch */
 	SswDevBuf d_items, d_bests, d_alns, d_res, d_colmax, d_tb, d_bnd, d_park, d_emul, d_grid, d_out, d_sync;
+	SswDevBuf d_hits;                                        /* ssw_engine_search: the n_q x k hit table of the grid path */
 	SswDevBuf d_mark;                                        /* ssw_engine_mark_mismatch: tasks, input CIGARs, marked CIGARs */
 	SswDevBuf d_rf_items, d_rf_bests, d_rf_blk, d_rf_cm;     /* block-maximum mode: re-fill items, their (unused) bests, first columns, column maxima */
 	SswStagedD2H staged;
@@ -339,7 +340,7 @@ extern "C" void ssw_engine_destroy(ssw_engine* e)
 {
 	if (!e) return;
 	cudaSetDevice(e->device);
-	SswDevBuf* bufs[] = {&e->d_q, &e->d_r, &e->d_mat, &e->d_items, &e->d_bests, &e->d_alns, &e->d_res, &e->d_colmax, &e->d_tb, &e->d_bnd, &e->d_park, &e->d_emul, &e->d_grid, &e->d_out, &e->d_sync, &e->d_rf_items, &e->d_rf_bests, &e->d_rf_blk, &e->d_rf_cm, &e->d_mark};
+	SswDevBuf* bufs[] = {&e->d_q, &e->d_r, &e->d_mat, &e->d_items, &e->d_bests, &e->d_alns, &e->d_res, &e->d_colmax, &e->d_tb, &e->d_bnd, &e->d_park, &e->d_emul, &e->d_grid, &e->d_out, &e->d_sync, &e->d_rf_items, &e->d_rf_bests, &e->d_rf_blk, &e->d_rf_cm, &e->d_mark, &e->d_hits};
 	for (SswDevBuf* b : bufs) b->release();
 	for (ssw_engine*& k : e->kids) if (k) { ssw_engine_destroy(k); k = nullptr; }
 	e->staged.release();
@@ -1328,10 +1329,18 @@ static int emul_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Aln>&
 /* ------------------------------------------------------------------------------------------- */
 
 
-/* Returns 1 when the grid path handled the batch (results filled; `redo` lists pairs to re-do by the general path),
- * 0 when the batch is not eligible, < 0 on error. */
+/* Top-k search on the grid path (ssw_engine_search): a selection kernel replaces the emit kernel, and an n_q x k hit table on the
+ * device replaces the n_pairs records.  Filled by grid_scores: each query's hits among the pairs that are final on the grid. */
+struct GridSearch {
+	int32_t k, min_score;                   /* min_score >= 1 */
+	std::vector<int32_t> hit_ref, n_hits;   /* n_q * k, n_q */
+	std::vector<ssw_batch_result> hits;     /* n_q * k */
+};
+
+/* Returns 1 when the grid path handled the batch (results filled -- or, with `gs`, the hit table; `redo` lists pairs to re-do
+ * by the general path), 0 when the batch is not eligible, < 0 on error. */
 static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, int64_t n_pairs,
-                       ssw_batch_result* results, std::vector<int32_t>* redo)
+                       ssw_batch_result* results, std::vector<int32_t>* redo, GridSearch* gs = nullptr)
 {
 	if (n_pairs != (int64_t)e->n_q * e->n_r || n_pairs < e->opt.grid_min_pairs || n_pairs > 0x7fffffff) return 0;
 	if (P.flag != 0 || P.gap_open <= P.gap_extend || e->opt.chunk != 0) return 0;
@@ -1375,7 +1384,9 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 	SSW_CUDA_OK(cudaMemcpyAsync(gb + o_rlen, e->r_len.data(), 4 * (size_t)n_r, cudaMemcpyHostToDevice, e->stream));
 	SSW_CUDA_OK(cudaMemcpyAsync(gb + o_cmp, cm_prefix.data(), 8 * (size_t)n_r, cudaMemcpyHostToDevice, e->stream));
 	SSW_CUDA_OK(cudaMemsetAsync(gb + o_cnt, 0, 256, e->stream));
-	if (e->d_out.ensure(sizeof(ssw_batch_result) * (size_t)n_pairs)) return -1;
+	/* search: [hits n_q*k][hit_ref n_q*k][n_hits n_q], every row written by the selection kernel of its query */
+	const size_t o_href = sizeof(ssw_batch_result) * (size_t)n_q * (gs ? gs->k : 0), o_nh = o_href + 4 * (size_t)n_q * (gs ? gs->k : 0);
+	if (gs ? e->d_hits.ensure(o_nh + 4 * (size_t)n_q) : e->d_out.ensure(sizeof(ssw_batch_result) * (size_t)n_pairs)) return -1;
 
 	const size_t free_b = ssw_free_device_bytes();
 	const size_t budget = std::max<size_t>((size_t)256 << 20, ssw_budget_share(free_b + e->d_colmax.cap + e->d_items.cap + e->d_alns.cap + e->d_res.cap));
@@ -1451,10 +1462,19 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 			ssw_launch(ssw_resolve_kernel<true>, dim3((unsigned)((n_desc + per - 1) / per)), dim3(SSW_RESOLVE_THREADS), 0, e->stream,
 			           (const SswAlnDesc*)e->d_alns.as<SswAlnDesc>(), (int)n_desc, (const SswItemBest*)e->d_bests.as<SswItemBest>(),
 			           (const uint32_t*)e->d_colmax.as<uint32_t>(), e->d_res.as<SswFillResult>());
-			ssw_launch(ssw_grid_emit_kernel, dim3((unsigned)((n_desc + 255) / 256)), dim3(256), 0, e->stream, A,
-			           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
-			           (const SswFillResult*)e->d_res.as<SswFillResult>(), e->d_out.as<ssw_batch_result>(),
-			           reinterpret_cast<int32_t*>(gb + o_list), reinterpret_cast<int32_t*>(gb + o_cnt), redo_cap);
+			if (!gs)
+				ssw_launch(ssw_grid_emit_kernel, dim3((unsigned)((n_desc + 255) / 256)), dim3(256), 0, e->stream, A,
+				           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
+				           (const SswFillResult*)e->d_res.as<SswFillResult>(), e->d_out.as<ssw_batch_result>(),
+				           reinterpret_cast<int32_t*>(gb + o_list), reinterpret_cast<int32_t*>(gb + o_cnt), redo_cap);
+			else {
+				uint8_t* hb = e->d_hits.as<uint8_t>();
+				ssw_launch(ssw_grid_select_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream, A,
+				           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
+				           (const SswFillResult*)e->d_res.as<SswFillResult>(), gs->k, gs->min_score,
+				           reinterpret_cast<int32_t*>(hb + o_href), reinterpret_cast<ssw_batch_result*>(hb), reinterpret_cast<int32_t*>(hb + o_nh),
+				           reinterpret_cast<int32_t*>(gb + o_list), reinterpret_cast<int32_t*>(gb + o_cnt), redo_cap);
+			}
 			SSW_CUDA_OK(cudaGetLastError());
 		}
 		e->laps.stop(e->stream, &e->timing.resolve_ms);
@@ -1491,7 +1511,15 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 	/* every launch is queued; bring the records back group by group on the copy stream while later groups still compute */
 	bool all_contiguous = !groups.empty();
 	for (const GridGroup& gg : groups) if (!gg.contiguous) all_contiguous = false;
-	if (all_contiguous && groups.size() > 1) {
+	if (gs) {
+		/* the hit table in one copy (rows of a rejected pilot group were overwritten by their second run) */
+		std::vector<uint8_t> h(o_nh + 4 * (size_t)n_q);
+		if (e->staged.copy(h.data(), e->d_hits.p, h.size(), e->stream)) return -1;
+		gs->hits.resize((size_t)n_q * gs->k); gs->hit_ref.resize((size_t)n_q * gs->k); gs->n_hits.resize((size_t)n_q);
+		memcpy(gs->hits.data(), h.data(), o_href);
+		memcpy(gs->hit_ref.data(), h.data() + o_href, o_nh - o_href);
+		memcpy(gs->n_hits.data(), h.data() + o_nh, 4 * (size_t)n_q);
+	} else if (all_contiguous && groups.size() > 1) {
 		if (!e->side[0]) SSW_CUDA_OK(cudaStreamCreateWithFlags(&e->side[0], cudaStreamNonBlocking));
 		for (const GridGroup& gg : groups) {
 			SSW_CUDA_OK(cudaStreamWaitEvent(e->side[0], gg.ev, 0));
@@ -1670,6 +1698,22 @@ static int align_general(ssw_engine* e, const ssw_batch_params& P, const Sem& S,
 	return 0;
 }
 
+/* scoring matrix on the device and the semantics it implies: bias = |min(mat)| for byte semantics (ssw.c:834-838) */
+static int prepare_scoring(ssw_engine* e, const ssw_batch_params& P, Sem* out)
+{
+	Sem& S = *out;
+	S.bias = 0; S.max_mat = -128;
+	for (int i = 0; i < P.n * P.n; ++i) { if (P.mat[i] < S.bias) S.bias = P.mat[i]; if (P.mat[i] > S.max_mat) S.max_mat = P.mat[i]; }
+	S.bias = S.bias < 0 ? -S.bias : S.bias;
+	S.limit_byte = 255 - S.bias;
+	S.limit_word = 32767 - std::max(S.max_mat, 0) - 256;
+	S.has_byte = P.score_size == 0 || P.score_size == 2;
+	S.has_word = P.score_size == 1 || P.score_size == 2;
+	if (e->d_mat.ensure((size_t)P.n * P.n + 16)) return -1;
+	SSW_CUDA_OK(cudaMemcpyAsync(e->d_mat.p, P.mat, (size_t)P.n * P.n, cudaMemcpyHostToDevice, e->stream));
+	return e->upload_refs(P.n);
+}
+
 static int engine_align_impl(ssw_engine* e, const ssw_batch_params* params,
                              int64_t n_pairs, const int32_t* pair_query, const int32_t* pair_ref,
                              ssw_batch_result* results,
@@ -1689,18 +1733,8 @@ static int engine_align_impl(ssw_engine* e, const ssw_batch_params* params,
 	if (n_pairs == 0) return 0;
 	e->t_total.start(e->stream);
 
-	/* scoring matrix: bias = |min(mat)| for byte semantics (ssw.c:834-838) */
 	Sem S;
-	S.bias = 0; S.max_mat = -128;
-	for (int i = 0; i < P.n * P.n; ++i) { if (P.mat[i] < S.bias) S.bias = P.mat[i]; if (P.mat[i] > S.max_mat) S.max_mat = P.mat[i]; }
-	S.bias = S.bias < 0 ? -S.bias : S.bias;
-	S.limit_byte = 255 - S.bias;
-	S.limit_word = 32767 - std::max(S.max_mat, 0) - 256;
-	S.has_byte = P.score_size == 0 || P.score_size == 2;
-	S.has_word = P.score_size == 1 || P.score_size == 2;
-	if (e->d_mat.ensure((size_t)P.n * P.n + 16)) return -1;
-	SSW_CUDA_OK(cudaMemcpyAsync(e->d_mat.p, P.mat, (size_t)P.n * P.n, cudaMemcpyHostToDevice, e->stream));
-	if (e->upload_refs(P.n)) return -1;
+	if (prepare_scoring(e, P, &S)) return -1;
 
 	int rc = 0;
 	/* Long reads with CIGARs: the banded traceback is a set of long serial chains that leaves most of the device idle, and
@@ -1833,6 +1867,136 @@ extern "C" int ssw_engine_align(ssw_engine* e, const ssw_batch_params* params,
 	/* nothing may unwind through the C ABI (std::bad_alloc from the planners' vectors, std::length_error, ...) */
 	try { SswBusyGuard busy(e ? e->device : 0); return engine_align_impl(e, params, n_pairs, pair_query, pair_ref, results, cigar_pool, pool_cap, pool_used); }
 	catch (const std::exception& ex) { fprintf(stderr, "[libssw-b200] ssw_engine_align: %s\n", ex.what()); return -1; }
+	catch (...) { return -1; }
+}
+
+/* ------------------------------------------------------------------------------------------- */
+/* top-k search over the full grid                                                               */
+/* ------------------------------------------------------------------------------------------- */
+
+struct SearchHit { int32_t r; ssw_batch_result rec; };
+
+/* the rank order of ssw_engine_search: status-1 pairs first (their score is at least the byte limit), then score1 descending,
+ * then reference ascending -- a total order, so the k best do not depend on how the grid was cut */
+static bool hit_before(const SearchHit& a, const SearchHit& b)
+{
+	if (a.rec.status != b.rec.status) return a.rec.status > b.rec.status;
+	if (a.rec.score1 != b.rec.score1) return a.rec.score1 > b.rec.score1;
+	return a.r < b.r;
+}
+static bool is_hit(const ssw_batch_result& o, int32_t min_score) { return o.status == 1 || o.score1 >= min_score; }
+
+/* the first k of v in rank order, sorted */
+static void keep_best(std::vector<SearchHit>& v, int32_t k)
+{
+	if ((int64_t)v.size() > k) { std::partial_sort(v.begin(), v.begin() + k, v.end(), hit_before); v.resize((size_t)k); }
+	else std::sort(v.begin(), v.end(), hit_before);
+}
+
+/* general path of a search: pairs per block of whole queries */
+#define SSW_SEARCH_BLOCK_PAIRS ((int64_t)1 << 22)
+
+static int engine_search_impl(ssw_engine* e, const ssw_batch_params* params, int32_t k, int32_t min_score,
+                              int32_t* hit_ref, ssw_batch_result* hits, int32_t* n_hits,
+                              uint32_t* cigar_pool, int64_t pool_cap, int64_t* pool_used)
+{
+	if (!e || !params || !params->mat) { fprintf(stderr, "[libssw-b200] ssw_engine_search: no engine or no parameters\n"); return -1; }
+	if (k < 1 || k > SSW_SEARCH_MAX_K) { fprintf(stderr, "[libssw-b200] ssw_engine_search: k = %d outside 1 .. %d\n", k, SSW_SEARCH_MAX_K); return -1; }
+	if (!hit_ref || !hits || !n_hits) { fprintf(stderr, "[libssw-b200] ssw_engine_search: NULL output array\n"); return -1; }
+	if (e->n_q <= 0 || e->n_r <= 0) { fprintf(stderr, "[libssw-b200] ssw_engine_search: no resident sequences\n"); return -1; }
+	const ssw_batch_params& P = *params;
+	if (P.n < 1 || P.n > 64) { fprintf(stderr, "[libssw-b200] alphabet size %d not supported (1..64)\n", P.n); return -1; }
+	int64_t pool_used_local = 0, no_pool = 0;
+	if (!pool_used) pool_used = &pool_used_local;
+	*pool_used = 0;
+	SSW_CUDA_OK(cudaSetDevice(e->device));
+	memset(&e->timing, 0, sizeof(e->timing));
+	e->laps.laps.clear(); e->laps.used = 0;
+	e->t_total.start(e->stream);
+	Sem S;
+	if (prepare_scoring(e, P, &S)) return -1;
+	const int32_t n_q = e->n_q, n_r = e->n_r, thr = std::max(min_score, 1);
+	/* the ranking runs on flag-0 records: score1, the ends and the second best do not depend on the flag */
+	ssw_batch_params P0 = P;
+	P0.flag = 0;
+	std::vector<std::vector<SearchHit>> best((size_t)n_q);
+	GridSearch gs;
+	gs.k = k; gs.min_score = thr;
+	std::vector<int32_t> redo;
+	int rc = grid_scores(e, P0, S, (int64_t)n_q * n_r, nullptr, &redo, &gs);
+	if (rc < 0) return rc;
+	if (rc == 1) {
+		for (int32_t q = 0; q < n_q; ++q)
+			for (int32_t i = 0; i < gs.n_hits[q]; ++i) best[q].push_back(SearchHit{gs.hit_ref[(size_t)q * k + i], gs.hits[(size_t)q * k + i]});
+		/* pairs the grid left to the general path, merged per query: the k best of all pairs are the k best of the grid's k best
+		 * and the re-done pairs, whatever the reason of the re-do */
+		if (!redo.empty()) {
+			std::vector<int32_t> pq(redo.size()), pr(redo.size());
+			for (size_t i = 0; i < redo.size(); ++i) { pq[i] = redo[i] / n_r; pr[i] = redo[i] % n_r; }
+			std::vector<ssw_batch_result> sub(redo.size());
+			const ssw_engine_timing keep = e->timing;
+			rc = align_general(e, P0, S, (int64_t)redo.size(), pq.data(), pr.data(), sub.data(), nullptr, 0, &no_pool);
+			if (rc) return rc;
+			e->timing.byte_overflows = keep.byte_overflows + (int64_t)redo.size();
+			for (size_t i = 0; i < redo.size(); ++i) if (is_hit(sub[i], thr)) best[pq[i]].push_back(SearchHit{pr[i], sub[i]});
+			for (int32_t q = 0; q < n_q; ++q) keep_best(best[q], k);
+		}
+	} else {
+		/* any other resident set: the general path on blocks of whole queries, the selection on the host */
+		const int32_t per = (int32_t)std::max<int64_t>(1, std::min<int64_t>(n_q, SSW_SEARCH_BLOCK_PAIRS / n_r));
+		std::vector<int32_t> pq, pr;
+		std::vector<ssw_batch_result> rec;
+		for (int32_t q0 = 0; q0 < n_q; q0 += per) {
+			const int32_t q1 = std::min(n_q, q0 + per);
+			const int64_t m = (int64_t)(q1 - q0) * n_r;
+			pq.resize((size_t)m); pr.resize((size_t)m); rec.resize((size_t)m);
+			for (int64_t i = 0; i < m; ++i) { pq[i] = q0 + (int32_t)(i / n_r); pr[i] = (int32_t)(i % n_r); }
+			const int64_t over = e->timing.byte_overflows;
+			e->timing.byte_overflows = 0;
+			rc = align_general(e, P0, S, m, pq.data(), pr.data(), rec.data(), nullptr, 0, &no_pool);
+			if (rc) return rc;
+			e->timing.byte_overflows += over;
+			for (int64_t i = 0; i < m; ++i) if (is_hit(rec[i], thr)) best[pq[i]].push_back(SearchHit{pr[i], rec[i]});
+			for (int32_t q = q0; q < q1; ++q) keep_best(best[q], k);
+		}
+	}
+	/* the caller's flag: begins and CIGARs of the hits only (at most n_q * k pairs) */
+	if (P.flag != 0) {
+		std::vector<int32_t> hq, hr;
+		for (int32_t q = 0; q < n_q; ++q) for (const SearchHit& h : best[q]) { hq.push_back(q); hr.push_back(h.r); }
+		if (!hq.empty()) {
+			std::vector<ssw_batch_result> rec(hq.size());
+			const int64_t over = e->timing.byte_overflows;
+			rc = align_general(e, P, S, (int64_t)hq.size(), hq.data(), hr.data(), rec.data(), cigar_pool, pool_cap, pool_used);
+			if (rc) return rc;
+			e->timing.byte_overflows = over;
+			size_t j = 0;
+			for (int32_t q = 0; q < n_q; ++q) for (SearchHit& h : best[q]) h.rec = rec[j++];
+		}
+	}
+	ssw_batch_result none;
+	memset(&none, 0, sizeof(none));
+	none.ref_begin1 = -1; none.read_begin1 = -1; none.cigar_off = -1;
+	for (int32_t q = 0; q < n_q; ++q) {
+		const std::vector<SearchHit>& v = best[q];
+		n_hits[q] = (int32_t)v.size();
+		for (int32_t i = 0; i < k; ++i) {
+			const bool used = i < (int32_t)v.size();
+			hit_ref[(size_t)q * k + i] = used ? v[i].r : -1;
+			hits[(size_t)q * k + i] = used ? v[i].rec : none;
+		}
+	}
+	e->timing.total_ms = e->t_total.stop(e->stream);
+	e->laps.collect();
+	return 0;
+}
+
+extern "C" int ssw_engine_search(ssw_engine* e, const ssw_batch_params* params, int32_t k, int32_t min_score,
+                                 int32_t* hit_ref, ssw_batch_result* hits, int32_t* n_hits,
+                                 uint32_t* cigar_pool, int64_t pool_cap, int64_t* pool_used)
+{
+	try { SswBusyGuard busy(e ? e->device : 0); return engine_search_impl(e, params, k, min_score, hit_ref, hits, n_hits, cigar_pool, pool_cap, pool_used); }
+	catch (const std::exception& ex) { fprintf(stderr, "[libssw-b200] ssw_engine_search: %s\n", ex.what()); return -1; }
 	catch (...) { return -1; }
 }
 

@@ -291,6 +291,102 @@ extern "C" int ssw_group_align(ssw_group* g, const ssw_batch_params* params, con
 	catch (...) { return -1; }
 }
 
+extern "C" int ssw_group_search(ssw_group* g, const ssw_batch_params* params, const int8_t* table, int32_t add_reverse_complement,
+                                int32_t n_queries, const void* queries, const int64_t* query_off,
+                                int32_t n_refs, const void* refs, const int64_t* ref_off,
+                                int32_t k, int32_t min_score, int32_t* hit_ref, ssw_batch_result* hits, int32_t* n_hits,
+                                uint32_t* cigar_pool, int64_t pool_cap, int64_t* pool_used)
+{
+	if (!g || g->eng.empty() || !params || !params->mat || !hit_ref || !hits || !n_hits) { fprintf(stderr, "[libssw-b200] ssw_group_search: NULL argument\n"); return -1; }
+	if (k < 1 || k > 1024) { fprintf(stderr, "[libssw-b200] ssw_group_search: k = %d outside 1 .. 1024\n", k); return -1; }
+	if (n_queries <= 0 || n_refs <= 0 || !queries || !refs || !query_off || !ref_off) { fprintf(stderr, "[libssw-b200] ssw_group_search: no sequences\n"); return -1; }
+	try {
+		if (pool_used) *pool_used = 0;
+		const ssw_batch_params& P = *params;
+		for (int32_t q = 0; q < n_queries; ++q) if (query_off[q + 1] < query_off[q]) { fprintf(stderr, "[libssw-b200] query offsets are not non-decreasing at %d\n", q); return -1; }
+		for (int32_t r = 0; r < n_refs; ++r) if (ref_off[r + 1] < ref_off[r]) { fprintf(stderr, "[libssw-b200] reference offsets are not non-decreasing at %d\n", r); return -1; }
+		const bool add_rc = table && add_reverse_complement;
+		const bool want_cigar = (P.flag & 7) != 0;
+		int64_t max_rl = 0;
+		for (int32_t r = 0; r < n_refs; ++r) max_rl = std::max<int64_t>(max_rl, ref_off[r + 1] - ref_off[r]);
+		/* the queries cut as for a full grid (ssw_group_align); every device searches its block against all references */
+		const int world = (int)g->eng.size();
+		const std::vector<int64_t> b = balanced_bounds(n_queries, world, [&](int64_t q) { return query_off[q + 1] - query_off[q] + 1; });
+		struct Part {
+			int32_t q0 = 0, n = 0;       /* first query; rows searched (queries, then their reverse complements) */
+			std::vector<int32_t> ref, nh;
+			std::vector<ssw_batch_result> rec;
+			std::unique_ptr<uint32_t[]> pool;
+			int64_t used = 0;
+			int rc = 0;
+		};
+		std::vector<Part> parts((size_t)world);
+		auto work = [&](int d) {
+			Part& S = parts[d];
+			try {
+				S.q0 = (int32_t)b[d];
+				const int32_t nq = (int32_t)(b[d + 1] - b[d]);
+				if (nq <= 0) return;
+				std::vector<int64_t> qoff((size_t)nq + 1);
+				for (int32_t j = 0; j <= nq; ++j) qoff[j] = query_off[S.q0 + j] - query_off[S.q0];
+				const char* qbase = (const char*)queries + query_off[S.q0];
+				ssw_engine* e = g->eng[d];
+				S.rc = table ? ssw_engine_set_sequences_text(e, nq, qbase, qoff.data(), n_refs, (const char*)refs, ref_off, table, P.n, add_rc ? 1 : 0)
+				             : ssw_engine_set_sequences(e, nq, (const int8_t*)qbase, qoff.data(), n_refs, (const int8_t*)refs, ref_off);
+				if (S.rc) return;
+				S.n = nq * (add_rc ? 2 : 1);
+				int64_t cap = 0;
+				if (want_cigar) for (int32_t j = 0; j < nq; ++j) cap += (int64_t)k * cigar_bound(qoff[j + 1] - qoff[j], max_rl, P.gap_extend);
+				if (add_rc) cap *= 2;
+				S.ref.resize((size_t)S.n * k); S.rec.resize((size_t)S.n * k); S.nh.resize((size_t)S.n);
+				S.pool.reset(new uint32_t[(size_t)cap + 8]);
+				S.rc = ssw_engine_search(e, &P, k, min_score, S.ref.data(), S.rec.data(), S.nh.data(), S.pool.get(), cap + 8, &S.used);
+			}
+			catch (const std::exception& ex) { fprintf(stderr, "[libssw-b200] device group: %s\n", ex.what()); S.rc = -1; }
+			catch (...) { S.rc = -1; }
+		};
+#ifdef SSW_CPU_EMU
+		for (int d = 0; d < world; ++d) work(d);        /* the emulator's fibers are not thread-safe */
+#else
+		{
+			std::vector<std::thread> th;
+			th.reserve((size_t)world);
+			for (int d = 1; d < world; ++d) {
+				try { th.emplace_back(work, d); }
+				catch (...) { work(d); }                 /* no thread to be had: this block runs here */
+			}
+			work(0);
+			for (std::thread& t : th) t.join();
+		}
+#endif
+		for (const Part& S : parts) if (S.rc) return S.rc;
+		int64_t base = 0;
+		for (const Part& S : parts) {
+			if (S.used > 0) {
+				if (!cigar_pool || base + S.used > pool_cap) { fprintf(stderr, "[libssw-b200] CIGAR pool too small\n"); return -1; }
+				if (base + S.used > 0x7fffffff) { fprintf(stderr, "[libssw-b200] more than 2^31 CIGAR words in one batch: split the batch\n"); return -1; }
+				memcpy(cigar_pool + base, S.pool.get(), sizeof(uint32_t) * (size_t)S.used);
+			}
+			const int32_t nq = add_rc ? S.n / 2 : S.n;
+			for (int32_t l = 0; l < S.n; ++l) {
+				const int64_t row = l < nq ? (int64_t)S.q0 + l : (int64_t)n_queries + S.q0 + (l - nq);
+				n_hits[row] = S.nh[l];
+				for (int32_t i = 0; i < k; ++i) {
+					ssw_batch_result o = S.rec[(size_t)l * k + i];
+					if (o.cigar_off >= 0) o.cigar_off += (int32_t)base;
+					hits[row * k + i] = o;
+					hit_ref[row * k + i] = S.ref[(size_t)l * k + i];
+				}
+			}
+			base += S.used;
+		}
+		if (pool_used) *pool_used = base;
+		return 0;
+	}
+	catch (const std::exception& ex) { fprintf(stderr, "[libssw-b200] ssw_group_search: %s\n", ex.what()); return -1; }
+	catch (...) { return -1; }
+}
+
 extern "C" int ssw_group_align_batch(ssw_group* g, const ssw_batch_params* params, const int8_t* table, int32_t add_reverse_complement,
                                      int32_t n_queries, const void* queries, const int64_t* query_off,
                                      int32_t n_refs, const void* refs, const int64_t* ref_off,

@@ -244,6 +244,33 @@ class BatchAligner(object):
             raise RuntimeError("ssw_engine_align failed (%d)" % rv)
         return res, pool[: used.value]
 
+    def search(self, mat, n, k, min_score=0, gap_open=3, gap_extend=1, flag=0, filters=0, filterd=0, mask_len=-1, score_size=2):
+        """Top-k search of every resident query against all resident references (ssw_engine_search).  Returns
+        (hit_ref[n_q, k] int32, hits[n_q, k] RESULT_DTYPE, n_hits[n_q] int32, cigar_pool[uint32]): row q holds query q's
+        n_hits[q] best hits in rank order (status-1 pairs, then score1 descending, then reference ascending); unused slots
+        have hit_ref -1."""
+        f = self.lib.ssw_engine_search
+        f.argtypes = [ct.c_void_p, ct.POINTER(BatchParams), ct.c_int32, ct.c_int32, ct.POINTER(ct.c_int32), ct.c_void_p,
+                      ct.POINTER(ct.c_int32), ct.POINTER(ct.c_uint32), ct.c_int64, ct.POINTER(ct.c_int64)]
+        f.restype = ct.c_int
+        mat, matp = _i8(mat)
+        P = BatchParams(matp, n, gap_open, gap_extend, flag, filters, filterd, mask_len, score_size)
+        rows = max(int(k), 0)
+        hit_ref = np.empty((self.n_q, rows), dtype=np.int32)
+        hits = np.empty((self.n_q, rows), dtype=RESULT_DTYPE)
+        n_hits = np.empty(self.n_q, dtype=np.int32)
+        cap = 0
+        if (flag & 7) and self._lens is not None and len(self._lens[1]):
+            ql, rl = self._lens
+            cap = int(rows * np.sum(ql + np.minimum(int(rl.max()), ql * 128) + 4))
+        pool = np.empty(max(cap, 1), dtype=np.uint32)
+        used = ct.c_int64(0)
+        rv = f(self.h, ct.byref(P), int(k), int(min_score), hit_ref.ctypes.data_as(ct.POINTER(ct.c_int32)), hits.ctypes.data_as(ct.c_void_p),
+               n_hits.ctypes.data_as(ct.POINTER(ct.c_int32)), pool.ctypes.data_as(ct.POINTER(ct.c_uint32)), len(pool), ct.byref(used))
+        if rv:
+            raise RuntimeError("ssw_engine_search failed (%d)" % rv)
+        return hit_ref, hits, n_hits, pool[: used.value]
+
     def mark_mismatch(self, res, pool, pair_query=None, pair_ref=None):
         """mark_mismatch (ssw.c:1019-1074) for every CIGAR of a batch, on the device (ssw_engine_mark_mismatch): `res` / `pool`
         as returned by align() for the same pairs.  Returns (records with cigar_off / cigar_len pointing into the new pool,
@@ -394,3 +421,48 @@ class GroupAligner(object):
         if rv:
             raise RuntimeError("ssw_group_align failed (%d)" % rv)
         return (res, pool[: used.value], nm) if marked else (res, pool[: used.value])
+
+    def search(self, queries, refs, mat, n, k, min_score=0, gap_open=3, gap_extend=1, flag=0, filters=0, filterd=0, mask_len=-1,
+               score_size=2, table=None, add_reverse_complement=False):
+        """BatchAligner.search over the devices of the group (ssw_group_search): sequences as for align().  Returns
+        (hit_ref[n_q, k], hits[n_q, k] RESULT_DTYPE, n_hits[n_q], cigar_pool); with add_reverse_complement the rows of the
+        reverse complements follow those of the queries."""
+        f = self.lib.ssw_group_search
+        f.argtypes = [ct.c_void_p, ct.POINTER(BatchParams), ct.POINTER(ct.c_int8), ct.c_int32,
+                      ct.c_int32, ct.c_void_p, ct.POINTER(ct.c_int64), ct.c_int32, ct.c_void_p, ct.POINTER(ct.c_int64),
+                      ct.c_int32, ct.c_int32, ct.POINTER(ct.c_int32), ct.c_void_p, ct.POINTER(ct.c_int32),
+                      ct.POINTER(ct.c_uint32), ct.c_int64, ct.POINTER(ct.c_int64)]
+        f.restype = ct.c_int
+        mat, matp = _i8(mat)
+        P = BatchParams(matp, n, gap_open, gap_extend, flag, filters, filterd, mask_len, score_size)
+        if table is None:
+            qc, qo = concat(queries)
+            rc, ro = concat(refs)
+            tabp = None
+        else:
+            qs = [q.encode() if isinstance(q, str) else bytes(q) for q in queries]
+            rs = [r.encode() if isinstance(r, str) else bytes(r) for r in refs]
+            qc = np.frombuffer(b"".join(qs) + b"\0", dtype=np.uint8)
+            rc = np.frombuffer(b"".join(rs) + b"\0", dtype=np.uint8)
+            qo = np.zeros(len(qs) + 1, dtype=np.int64); qo[1:] = np.cumsum([len(q) for q in qs])
+            ro = np.zeros(len(rs) + 1, dtype=np.int64); ro[1:] = np.cumsum([len(r) for r in rs])
+            tab = np.ascontiguousarray(table, dtype=np.int8)
+            assert tab.size == 128
+            tabp = tab.ctypes.data_as(ct.POINTER(ct.c_int8))
+        ql, rl = np.diff(qo), np.diff(ro)
+        if table is not None and add_reverse_complement:
+            ql = np.concatenate([ql, ql])
+        rows = max(int(k), 0)
+        hit_ref = np.empty((len(ql), rows), dtype=np.int32)
+        hits = np.empty((len(ql), rows), dtype=RESULT_DTYPE)
+        n_hits = np.empty(len(ql), dtype=np.int32)
+        cap = int(rows * np.sum(ql + np.minimum(int(rl.max()), ql * 128) + 4)) if (flag & 7) and len(rl) else 0
+        pool = np.empty(max(cap, 1), dtype=np.uint32)
+        used = ct.c_int64(0)
+        rv = f(self.h, ct.byref(P), tabp, 1 if add_reverse_complement else 0, len(queries), qc.ctypes.data_as(ct.c_void_p),
+               qo.ctypes.data_as(ct.POINTER(ct.c_int64)), len(refs), rc.ctypes.data_as(ct.c_void_p), ro.ctypes.data_as(ct.POINTER(ct.c_int64)),
+               int(k), int(min_score), hit_ref.ctypes.data_as(ct.POINTER(ct.c_int32)), hits.ctypes.data_as(ct.c_void_p),
+               n_hits.ctypes.data_as(ct.POINTER(ct.c_int32)), pool.ctypes.data_as(ct.POINTER(ct.c_uint32)), len(pool), ct.byref(used))
+        if rv:
+            raise RuntimeError("ssw_group_search failed (%d)" % rv)
+        return hit_ref, hits, n_hits, pool[: used.value]

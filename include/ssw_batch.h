@@ -101,6 +101,23 @@ int ssw_engine_align(ssw_engine* e, const ssw_batch_params* params,
                      uint32_t* cigar_pool, int64_t pool_cap, int64_t* pool_used);
 
 /*
+ * Top-k search of the resident queries against the resident references (full grid). Hits of query q are at
+ * [q*k, q*k + n_hits[q]) of hit_ref / hits, in rank order; unused slots have hit_ref = -1.
+ *   hit        a pair with score1 >= max(min_score, 1), or a pair with status 1 (score_size 0, byte overflow: its score is
+ *              at least the byte limit; a hit whatever min_score is)
+ *   rank       status-1 pairs first, then score1 descending, then reference index ascending (a total order: the result does
+ *              not depend on the devices or on the path that ran)
+ *   records    field for field what ssw_engine_align returns for that pair with the same params; begins and CIGARs (flag & 7)
+ *              are computed for the hits only, into cigar_pool as ssw_engine_align fills it
+ *   k          1 .. 1024
+ * No record of the n_queries x n_refs grid crosses to the host: the k best of every query are selected on the device where
+ * the grid path can run (scores-only planning on the device), on the host per block of queries otherwise.
+ */
+int ssw_engine_search(ssw_engine* e, const ssw_batch_params* params, int32_t k, int32_t min_score,
+                      int32_t* hit_ref, ssw_batch_result* hits, int32_t* n_hits,
+                      uint32_t* cigar_pool, int64_t pool_cap, int64_t* pool_used);
+
+/*
  * mark_mismatch (ssw.h:157-164; ssw.c:1019-1074) for the CIGARs of a whole batch, on the device: for every record of
  * `results` that carries a CIGAR (words at cigar_pool[cigar_off ...]) the M runs are split into '=' and 'X' runs, soft
  * clips are added for the unaligned ends of the read, and nm[p] (may be NULL) receives the number of mismatching +
@@ -178,6 +195,16 @@ int ssw_group_align(ssw_group* g, const ssw_batch_params* params, const int8_t* 
                     ssw_batch_result* results, uint32_t* cigar_pool, int64_t pool_cap, int64_t* pool_used,
                     int32_t marked, int32_t* nm);
 
+/* ssw_engine_search over the devices of the group: the queries are cut as for a full grid, every device searches its block
+ * against all references, and its hit rows land in the caller's arrays (n_queries x k; with add_reverse_complement
+ * 2 * n_queries rows, the reverse complements after the queries).  The CIGAR words of the devices are concatenated
+ * (cigar_off re-based).  Results do not depend on the number of devices. */
+int ssw_group_search(ssw_group* g, const ssw_batch_params* params, const int8_t* table, int32_t add_reverse_complement,
+                     int32_t n_queries, const void* queries, const int64_t* query_off,
+                     int32_t n_refs, const void* refs, const int64_t* ref_off,
+                     int32_t k, int32_t min_score, int32_t* hit_ref, ssw_batch_result* hits, int32_t* n_hits,
+                     uint32_t* cigar_pool, int64_t pool_cap, int64_t* pool_used);
+
 /* The same with heap s_align records (ssw_align_batch / _text / _marked over a group); release with align_destroy. */
 int ssw_group_align_batch(ssw_group* g, const ssw_batch_params* params, const int8_t* table, int32_t add_reverse_complement,
                           int32_t n_queries, const void* queries, const int64_t* query_off,
@@ -185,7 +212,8 @@ int ssw_group_align_batch(ssw_group* g, const ssw_batch_params* params, const in
                           int64_t n_pairs, const int32_t* pair_query, const int32_t* pair_ref,
                           s_align** out, int32_t marked, int32_t* nm);
 
-/* Device-time breakdown of the last ssw_engine_align call (CUDA events on the engine's stream), in ms. */
+/* Device-time breakdown of the last ssw_engine_align / ssw_engine_search call (CUDA events on the engine's stream), in ms.
+ * A search counts its selection kernels in other_launches / resolve_ms. */
 typedef struct {
 	float fill_forward_ms;   /* matrix fill kernels, forward pass (incl. byte->word reruns) */
 	float resolve_ms;        /* bookkeeping kernels */
