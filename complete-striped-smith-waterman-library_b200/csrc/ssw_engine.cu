@@ -219,10 +219,11 @@ struct FillPtrs { const SswItem* items; uint32_t* cm; SswItemBest* bests; bool a
 /* Warps per CTA and dynamic shared memory of a fill launch with R rows per lane for an alphabet of n letters.  Per-warp
  * profiles (share == 0) can be large for big alphabets: fewer warps per CTA then.  A forward launch with a CTA-shared
  * profile takes 8 warps instead of 4 when that doubles the resident warps per SM (large alphabets: the profile, not the
- * registers, limits the CTAs per SM). */
+ * registers, limits the CTAs per SM).  track == false (block mode, CM == 2, keeps no best cell): no snapshot area; the warp
+ * count stays the one chosen with it, so that the planner's items per CTA do not depend on the column-maximum mode. */
 struct FillShape { int warps; size_t smem; };
 template <int R>
-static FillShape fill_shape(int n, int share, int dir)
+static FillShape fill_shape(int n, int share, int dir, bool track = true)
 {
 	const size_t prof = ssw_fill_smem_bytes<R>(n, 1), snap = ssw_snap_smem_bytes<R>(32);
 	int warps = SSW_FILL_WARPS;
@@ -232,7 +233,7 @@ static FillShape fill_shape(int n, int share, int dir)
 		const int occ4 = (int)std::min<size_t>(SSW_FILL_MINB, sm / s4), occ8 = (int)std::min<size_t>(2, sm / s8);
 		if (occ8 * 8 > occ4 * 4) warps = 8;
 	}
-	return FillShape{warps, (share ? prof : prof * warps) + snap * warps};       /* profile(s), then the best-cell snapshots */
+	return FillShape{warps, (share ? prof : prof * warps) + (track ? snap * warps : 0)};       /* profile(s), then the best-cell snapshots */
 }
 
 /* items per CTA of a forward launch of instance `inst` with CTA-shared profiles */
@@ -244,7 +245,7 @@ static int fill_items_per_cta(int inst, int n)
 template <int G, int R>
 static int launch_fill(ssw_engine* e, const FillPtrs& fp, int n_items, int dir, int cm_mode, int share, const ssw_batch_params& P)
 {
-	const FillShape sh = fill_shape<R>(P.n, share, dir);
+	const FillShape sh = fill_shape<R>(P.n, share, dir, !(dir > 0 && cm_mode == 2));
 	if (sh.smem > 220 * 1024) { fprintf(stderr, "[libssw-b200] alphabet of %d letters is too large for this query length\n", P.n); return -2; }
 	const int per_cta = sh.warps * (32 / G);
 	const int grid = (n_items + per_cta - 1) / per_cta;
@@ -298,17 +299,18 @@ int ssw_engine::run_fill(const std::vector<SswItem>& items, int inst, int dir, i
 }
 
 
-/* resident CTAs per SM of the forward fill kernel of instance `inst` in CTA-shared-profile mode */
-static int fill_occupancy(int inst, int n)
+/* resident CTAs per SM of the forward fill kernel of instance `inst` in CTA-shared-profile mode (block: with the shared
+ * memory of a block-mode launch, which has no snapshot area) */
+static int fill_occupancy(int inst, int n, bool block)
 {
-	static int cache[kNumInst][65];
+	static int cache[kNumInst][65][2];
 	static std::mutex mu;
 	if (inst < 0 || inst >= kNumInst || n < 0 || n > 64) return 1;
 	std::lock_guard<std::mutex> lock(mu);
-	int& occ = cache[inst][n];
-	if (!occ) occ = std::max(1, visit_inst(inst, [n](auto t) {
+	int& occ = cache[inst][n][block ? 1 : 0];
+	if (!occ) occ = std::max(1, visit_inst(inst, [n, block](auto t) {
 		using T = decltype(t);
-		const FillShape sh = fill_shape<T::R>(n, 1, +1);
+		const FillShape sh = fill_shape<T::R>(n, 1, +1, !block);
 		auto kern = ssw_fill_kernel<T::G, T::R, 1, 2, false, SSW_FILL_WARPS, false>;
 		if constexpr (T::R >= 16) if (sh.warps == 8) kern = ssw_fill_kernel<T::G, T::R, 1, 2, false, 8, false>;
 		ssw_ensure_dyn_smem(reinterpret_cast<const void*>(kern), sh.smem);
@@ -665,24 +667,33 @@ static int run_resolve(ssw_engine* e, const std::vector<SswAlnDesc>& descs, bool
 	e->laps.start(e->stream);
 	const int per = SSW_RESOLVE_THREADS / 32;
 	const dim3 grid(((int)descs.size() + per - 1) / per);
-	if (second && cm && cm->block) {
-		/* block maxima: stage 1 (summaries + the three blocks per alignment that need single columns, and the columns right of
-		 * the mask window of byte alignments filled on their word rows), re-fill of those ranges with one word per column, stage 2 */
-		const size_t n_rf = descs.size() * SSW_REFILL_SLOTS;
-		if (e->d_rf_items.ensure(sizeof(SswItem) * n_rf)) return -1;
-		if (e->d_rf_bests.ensure(sizeof(SswItemBest) * n_rf)) return -1;
+	if (cm && cm->block) {
+		/* block maxima (the fill kept no item bests, so this runs whether or not the second best is wanted): stage 0 (the first
+		 * block holding the score) and its re-fill with best-cell tracking, stage 1 (the best cell + the three blocks per
+		 * alignment that need single columns, and the columns right of the mask window of byte alignments filled on their word
+		 * rows), re-fill of those ranges with one word per column, stage 2.  Scratch: SSW_REFILL_SLOTS items per alignment,
+		 * then one best-block item per alignment. */
+		const size_t n_aln = descs.size(), n_rf = n_aln * SSW_REFILL_SLOTS;
+		if (e->d_rf_items.ensure(sizeof(SswItem) * (n_rf + n_aln))) return -1;
+		if (e->d_rf_bests.ensure(sizeof(SswItemBest) * (n_rf + n_aln))) return -1;
 		if (e->d_rf_blk.ensure(sizeof(int32_t) * n_rf)) return -1;    /* first column of every re-filled range, -1: none */
 		if (e->d_rf_cm.ensure(sizeof(uint32_t) * n_rf * SSW_CM_BLOCK + 64)) return -1;
+		ssw_launch(ssw_resolve_best_block_kernel<0>, grid, dim3(SSW_RESOLVE_THREADS), 0, e->stream, (const SswAlnDesc*)e->d_alns.as<SswAlnDesc>(),
+		           (int)n_aln, (const uint32_t*)e->d_colmax.as<uint32_t>(), (const SswItem*)e->d_items.as<SswItem>(), e->d_rf_items.as<SswItem>() + n_rf);
+		SSW_CUDA_OK(cudaGetLastError());
+		const FillPtrs fp_best = {e->d_rf_items.as<SswItem>() + n_rf, e->d_rf_cm.as<uint32_t>(), e->d_rf_bests.as<SswItemBest>() + n_rf};
+		int rc = dispatch_fill(e, cm->inst, fp_best, (int)n_aln, +1, 1, 0, *cm->P);
+		if (rc) return rc < 0 ? rc : -1;
 		ssw_launch(ssw_resolve_blocks_kernel<0>, grid, dim3(SSW_RESOLVE_THREADS), 0, e->stream, (const SswAlnDesc*)e->d_alns.as<SswAlnDesc>(),
-		           (int)descs.size(), (const SswItemBest*)e->d_bests.as<SswItemBest>(), (const uint32_t*)e->d_colmax.as<uint32_t>(),
+		           (int)n_aln, (const SswItemBest*)e->d_rf_bests.as<SswItemBest>() + n_rf, (const uint32_t*)e->d_colmax.as<uint32_t>(),
 		           (const SswItem*)e->d_items.as<SswItem>(), e->d_res.as<SswFillResult>(), e->d_rf_items.as<SswItem>(), e->d_rf_blk.as<int32_t>());
 		SSW_CUDA_OK(cudaGetLastError());
 		const FillPtrs fp = {e->d_rf_items.as<SswItem>(), e->d_rf_cm.as<uint32_t>(), e->d_rf_bests.as<SswItemBest>()};
-		const int rc = dispatch_fill(e, cm->inst, fp, (int)n_rf, +1, 1, 0, *cm->P);
+		rc = dispatch_fill(e, cm->inst, fp, (int)n_rf, +1, 1, 0, *cm->P);
 		if (rc) return rc < 0 ? rc : -1;
 		ssw_launch(ssw_resolve_refill_kernel<0>, grid, dim3(SSW_RESOLVE_THREADS), 0, e->stream, (const SswAlnDesc*)e->d_alns.as<SswAlnDesc>(),
-		           (int)descs.size(), (const int32_t*)e->d_rf_blk.as<int32_t>(), (const uint32_t*)e->d_rf_cm.as<uint32_t>(), e->d_res.as<SswFillResult>());
-		e->timing.other_launches += 2;
+		           (int)n_aln, (const int32_t*)e->d_rf_blk.as<int32_t>(), (const uint32_t*)e->d_rf_cm.as<uint32_t>(), e->d_res.as<SswFillResult>());
+		e->timing.other_launches += 4;
 	} else if (second)
 		ssw_launch(ssw_resolve_kernel<true>, grid, dim3(SSW_RESOLVE_THREADS), 0, e->stream, (const SswAlnDesc*)e->d_alns.as<SswAlnDesc>(),
 		           (int)descs.size(), (const SswItemBest*)e->d_bests.as<SswItemBest>(), (const uint32_t*)e->d_colmax.as<uint32_t>(), e->d_res.as<SswFillResult>());
@@ -1107,7 +1118,7 @@ static int forward_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Al
 		 * (fill of the last wave) x (1 - warm-up overhead). */
 		int64_t auto_chunk = base_chunk;
 		if (e->opt.chunk == 0 && base_chunk >= 4096) {
-			const int occ = fill_occupancy(inst, P.n);
+			const int occ = fill_occupancy(inst, P.n, block);
 			const double slots = (double)e->sm_count * std::max(occ, 1);
 			double best_eff = -1;
 			for (int pct = 60; pct <= 150; pct += 5) {

@@ -29,10 +29,11 @@
  *                           from a boundary buffer a few columns behind its producer.
  *
  * Outputs per item: the lexicographic best cell (score, first scan position,
- * smallest row) per half, and -- forward pass -- the column maxima over real
- * and pad rows (the reference's maxColumn[], ssw.c:338/:540) as packed s16x2
- * words.  All order-dependent semantics (strict '>' running maximum, byte
- * overflow, mask window) are applied afterwards by ssw_resolve.cuh.
+ * smallest row) per half -- not in block mode (CM == 2) -- and, forward pass,
+ * the column maxima over real and pad rows (the reference's maxColumn[],
+ * ssw.c:338/:540) as packed s16x2 words.  All order-dependent semantics (strict
+ * '>' running maximum, byte overflow, mask window) are applied afterwards by
+ * ssw_resolve.cuh.
  */
 #ifndef SSW_FILL_CUH
 #define SSW_FILL_CUH
@@ -342,9 +343,10 @@ __device__ static __forceinline__ void ssw_reduce_best(const SswLaneBest& lb, in
 /* CM: what the forward pass records of the column maxima (the reference's maxColumn[], ssw.c:338/:540)
  *   0  nothing (reverse pass)
  *   1  every column: one packed word per reference column (short references, the re-fill items of mode 2)
- *   2  one packed word per block of SSW_CM_BLOCK columns.  The second-best scan (ssw.c:368-381) needs single columns
- *      only in the <= 2 blocks cut by the mask window and in the block that holds the winner; ssw_resolve.cuh
- *      re-fills those three blocks per alignment with mode 1.  Chunks start at multiples of SSW_CM_BLOCK. */
+ *   2  one packed word per block of SSW_CM_BLOCK columns, and no best cell (`bests` is not written).  The best cell needs
+ *      single columns only in the first block holding the largest block maximum, the second-best scan (ssw.c:368-381) only
+ *      in the <= 2 blocks cut by the mask window and in the block that holds the winner; ssw_resolve.cuh re-fills those
+ *      blocks per alignment with mode 1.  Chunks start at multiples of SSW_CM_BLOCK. */
 /* WARPS: warps per CTA.  4 by default; 8 where one CTA-shared profile is so large (protein alphabets: 64 KB at 20 rows per
  * lane) that four-warp CTAs would leave the SM with 8 resident warps -- eight warps per profile keep 16. */
 /* ARM: items may carry a late arming position (SswItem.cend, device-planned grids); a template parameter so that the kernels
@@ -418,15 +420,19 @@ ssw_fill_kernel(const SswItem* __restrict__ items, int n_items,
 #pragma unroll
 	for (int k = 0; k < R; ++k) { Hd[k] = 0; E[k] = 0; }
 	uint32_t outH = 0, outF = 0, outC = 0;
+	/* Block mode keeps no best cell: the resolve takes the score and the first block holding it from the block maxima and
+	 * re-fills that one block with tracking (ssw_resolve.cuh).  So its sweep carries only the recurrence and the maxima. */
+	constexpr bool TRACK = CM != 2;
 	SswLaneBest lb;
 	lb.best = 0; lb.pos0 = lb.pos1 = -1; lb.row0 = lb.row1 = 0;      /* position -1: no recorded event (yet) */
 	SswSnap<R> snap;
-	ssw_snap_init<R>(snap, reinterpret_cast<uint4*>(smem + (size_t)(share ? 1 : nwarps) * (size_t)(n + 1) * 32 * S), (int)threadIdx.x);
+	if constexpr (TRACK)
+		ssw_snap_init<R>(snap, reinterpret_cast<uint4*>(smem + (size_t)(share ? 1 : nwarps) * (size_t)(n + 1) * 32 * S), (int)threadIdx.x);
 	uint32_t blk_acc = 0;                               /* CM == 2: running maximum of the current block (last lane) */
 
 	for (int body = 0; body < n_body; ++body) {
 		uint32_t cmv[U];
-		if ((body & (SSW_FLOOR_PERIOD - 1)) == 0) {
+		if (TRACK && (body & (SSW_FLOOR_PERIOD - 1)) == 0) {
 			/* lower bound of the group's final maximum: a lane value below it can never be the best cell, so the lane's
 			 * running best is raised to (bound - 1) and such values no longer trigger the bookkeeping */
 			const uint32_t floor2 = ssw_group_max<G>(lb.best);
@@ -455,11 +461,13 @@ ssw_fill_kernel(const SswItem* __restrict__ items, int n_items,
 			cmv[j] = outC;
 
 			/* running best of this lane's rows (strict increase only; rare path) */
-			const uint32_t nb = __vmaxs2(lb.best, own);
-			if (unarmed) lb.best = nb;
-			else if (nb != lb.best && maybe_counted) {
-				if (ARM && DIR > 0 && sp0 + j < it.cend) lb.best = nb;   /* the body that crosses `arm`: still before it */
-				else ssw_track<R>(lb, snap, nb, Hn, sp0 + j, it.p0, it.p1);
+			if constexpr (TRACK) {
+				const uint32_t nb = __vmaxs2(lb.best, own);
+				if (unarmed) lb.best = nb;
+				else if (nb != lb.best && maybe_counted) {
+					if (ARM && DIR > 0 && sp0 + j < it.cend) lb.best = nb;   /* the body that crosses `arm`: still before it */
+					else ssw_track<R>(lb, snap, nb, Hn, sp0 + j, it.p0, it.p1);
+				}
 			}
 		}
 
@@ -473,17 +481,15 @@ ssw_fill_kernel(const SswItem* __restrict__ items, int n_items,
 		}
 		if (CM == 2) {
 			/* p0 and sL are multiples of 8 here, so a body lies entirely before p0 or not at all; only the last body of the
-			 * reference can be cut by p1 (columns behind the reference must not count: E decays into the null pad) */
+			 * reference can be cut by p1 (chunks end at block boundaries).  Its columns behind the reference are folded in as
+			 * well: there the null letters leave X = max(0, E) with E(c) <= H(c-1) of the same row, and F only carries X down,
+			 * so such a column's maximum never exceeds that of the column before it -- the block maximum stays the same, and
+			 * the body needs no per-column predicates (which would be issued on every body). */
 			if (t == G - 1 && it.cm_off != SSW_CM_NONE && sL >= it.p0 && sL < it.p1) {
-				if (sL + U <= it.p1) {
-					blk_acc = __vimax3_s16x2(blk_acc, cmv[0], cmv[1]);
-					blk_acc = __vimax3_s16x2(blk_acc, cmv[2], cmv[3]);
-					blk_acc = __vimax3_s16x2(blk_acc, cmv[4], cmv[5]);
-					blk_acc = __vimax3_s16x2(blk_acc, cmv[6], cmv[7]);
-				} else {
-#pragma unroll
-					for (int j = 0; j < U; ++j) if (sL + j < it.p1) blk_acc = __vmaxs2(blk_acc, cmv[j]);
-				}
+				blk_acc = __vimax3_s16x2(blk_acc, cmv[0], cmv[1]);
+				blk_acc = __vimax3_s16x2(blk_acc, cmv[2], cmv[3]);
+				blk_acc = __vimax3_s16x2(blk_acc, cmv[4], cmv[5]);
+				blk_acc = __vimax3_s16x2(blk_acc, cmv[6], cmv[7]);
 				if (((sL + U) & (SSW_CM_BLOCK - 1)) == 0 || sL + U >= it.p1) {
 					colmax[it.cm_off + (sL / SSW_CM_BLOCK)] = blk_acc;
 					blk_acc = 0;
@@ -510,16 +516,18 @@ ssw_fill_kernel(const SswItem* __restrict__ items, int n_items,
 		}
 	}
 
-	ssw_track_rows<R>(lb, snap, t * R);
-	ssw_track_unrecorded(lb);
-	int sc0, bp0, br0, sc1, bp1, br1;
-	ssw_reduce_best<G>(lb, sc0, bp0, br0, sc1, bp1, br1);
-	if (live && t == 0) {
-		SswItemBest b;
-		b.score[0] = sc0; b.pos[0] = bp0; b.row[0] = br0;
-		b.score[1] = sc1; b.pos[1] = bp1; b.row[1] = br1;
-		b.p0 = it.p0; b.p1 = it.p1;
-		bests[item_idx] = b;
+	if constexpr (TRACK) {
+		ssw_track_rows<R>(lb, snap, t * R);
+		ssw_track_unrecorded(lb);
+		int sc0, bp0, br0, sc1, bp1, br1;
+		ssw_reduce_best<G>(lb, sc0, bp0, br0, sc1, bp1, br1);
+		if (live && t == 0) {
+			SswItemBest b;
+			b.score[0] = sc0; b.pos[0] = bp0; b.row[0] = br0;
+			b.score[1] = sc1; b.pos[1] = bp1; b.row[1] = br1;
+			b.p0 = it.p0; b.p1 = it.p1;
+			bests[item_idx] = b;
+		}
 	}
 }
 

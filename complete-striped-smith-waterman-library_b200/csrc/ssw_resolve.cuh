@@ -114,15 +114,18 @@ ssw_resolve_kernel(const SswAlnDesc* __restrict__ alns, int n_aln,
 /* block-maximum mode (fill kernel CM == 2): one word per SSW_CM_BLOCK columns instead of one per column       */
 /* ---------------------------------------------------------------------------------------------------------- */
 /*
+ * The block-mode fill keeps no best cell.  Its score is the largest block maximum, and its first column lies in the
+ * first block holding that value: stage 0 (ssw_resolve_best_block_kernel) finds that block and emits one re-fill item
+ * per alignment for it (the same pair-task, counted range = the block, warm-up as the chunks of the main launch), which
+ * the fill kernel (CM == 1) runs with its best-cell tracking: (score, first column, smallest row) of that block is the
+ * alignment's best cell.
  * The second-best scan wants (largest value, smallest column) over the columns outside the mask window.  With
- * block maxima that is known exactly for every item that does not touch the window (its best cell is the summary),
- * and per block for the others; single columns are needed only in
+ * block maxima that is known per block; single columns are needed only in
  *   - the block cut by the left edge of the window and the block cut by its right edge, and
  *   - the first block holding the largest block maximum among the fully allowed blocks (to find its first column).
- * Stage 1 (ssw_resolve_blocks_kernel) does everything ssw_resolve_kernel does, keeps the best exact candidate in
- * score2/ref2, and emits three re-fill items per alignment (dead ones where nothing is needed): the same pair-task,
- * counted range = one block, warm-up as the chunks of the main launch.  The fill kernel (CM == 1) writes their 64
- * column maxima into a small scratch; stage 2 (ssw_resolve_refill_kernel) folds them in.
+ * Stage 1 (ssw_resolve_blocks_kernel) does everything ssw_resolve_kernel does, with the best cell of stage 0, and
+ * emits three re-fill items per alignment (dead ones where nothing is needed), built like the one of stage 0.  The fill
+ * kernel (CM == 1) writes their 64 column maxima into a small scratch; stage 2 (ssw_resolve_refill_kernel) folds them in.
  * A byte alignment filled on its word rows (SswAlnDesc.byte_pad > 0) gets a fourth item: columns [e2, e2 + 8) on the
  * byte rows, the only allowed columns whose byte column maxima can exceed the word ones in a way the scan sees (DESIGN 2).
  * Its range starts at e2 rounded down to 4 (the 128-bit column stores of the fill); blocks 0..2 stay on the word rows,
@@ -131,10 +134,51 @@ ssw_resolve_kernel(const SswAlnDesc* __restrict__ alns, int n_aln,
 #define SSW_REFILL_SLOTS 4
 #define SSW_REFILL_ZONE 3       /* slot of the byte-row columns right of the mask window */
 
+/* re-fill item of columns [p0, p1) of the alignment's pair-task (p1 <= p0: a dead item), warm-up as in the main launch */
+__device__ static __forceinline__ SswItem ssw_refill_item(const SswAlnDesc& d, const SswItem* __restrict__ items, int p0, int p1)
+{
+	SswItem it = items[d.n_items > 0 ? d.first_item : 0];
+	it.term_a = -1; it.cend = 0; it.cm_off = SSW_CM_NONE;
+	if (p1 > p0) { it.p0 = p0; it.p1 = p1; it.warm = min(d.warm, p0); }     /* d.warm is taken from the byte padding */
+	else { it.p0 = it.p1 = 0; it.warm = 0; }
+	return it;
+}
+
+/* stage 0: the first block holding the largest block maximum of the alignment's half, as a re-fill item (dead when the
+ * score is 0).  The byte overflow test needs the score only, but the overflowed result keeps its position and row. */
+template <int DUMMY = 0>
+__global__ void __launch_bounds__(SSW_RESOLVE_THREADS)
+ssw_resolve_best_block_kernel(const SswAlnDesc* __restrict__ alns, int n_aln, const uint32_t* __restrict__ blkmax,
+                              const SswItem* __restrict__ items, SswItem* __restrict__ best_items)
+{
+	constexpr unsigned FULL = 0xffffffffu;
+	const int lane = threadIdx.x & 31;
+	const int idx = (int)blockIdx.x * (SSW_RESOLVE_THREADS / 32) + (threadIdx.x >> 5);
+	if (idx >= n_aln) return;
+	const SswAlnDesc d = alns[idx];
+	int vb = 0, bb = 0x7fffffff;
+	if (d.cm_off != SSW_CM_NONE && d.n_items > 0) {
+		const uint32_t* bm = blkmax + d.cm_off;
+		const int n_blk = (d.ref_len + SSW_CM_BLOCK - 1) / SSW_CM_BLOCK;
+		for (int b = lane; b < n_blk; b += 32) {
+			const int v = half_of(bm[b], d.half);
+			if (v > vb) { vb = v; bb = b; }
+		}
+	}
+#pragma unroll
+	for (int off = 16; off >= 1; off >>= 1) {
+		const int o_vb = __shfl_xor_sync(FULL, vb, off), o_bb = __shfl_xor_sync(FULL, bb, off);
+		if (o_vb > vb || (o_vb == vb && o_bb < bb)) { vb = o_vb; bb = o_bb; }
+	}
+	if (lane == 0) best_items[idx] = vb > 0 ? ssw_refill_item(d, items, bb * SSW_CM_BLOCK, min(bb * SSW_CM_BLOCK + SSW_CM_BLOCK, d.ref_len))
+	                                        : ssw_refill_item(d, items, 0, 0);
+}
+
+/* stage 1: `best` holds the re-fill record of stage 0's block, one per alignment */
 template <int DUMMY = 0>
 __global__ void __launch_bounds__(SSW_RESOLVE_THREADS)
 ssw_resolve_blocks_kernel(const SswAlnDesc* __restrict__ alns, int n_aln,
-                          const SswItemBest* __restrict__ bests, const uint32_t* __restrict__ blkmax,
+                          const SswItemBest* __restrict__ best, const uint32_t* __restrict__ blkmax,
                           const SswItem* __restrict__ items, SswFillResult* __restrict__ out,
                           SswItem* __restrict__ refill_items, int32_t* __restrict__ refill_c0)
 {
@@ -145,28 +189,15 @@ ssw_resolve_blocks_kernel(const SswAlnDesc* __restrict__ alns, int n_aln,
 	const SswAlnDesc d = alns[idx];
 	const int h = d.half;
 
-	int sc = 0, pos = 0x7fffffff, row = 0x7fffffff;
-	for (int k = lane; k < d.n_items; k += 32) {
-		const SswItemBest b = bests[d.first_item + k];
-		const int s = b.score[h], p = b.pos[h], rr = b.row[h];
-		if (s > 0 && (s > sc || (s == sc && (p < pos || (p == pos && rr < row))))) { sc = s; pos = p; row = rr; }
-	}
-#pragma unroll
-	for (int off = 16; off >= 1; off >>= 1) {
-		const int o_sc = __shfl_xor_sync(FULL, sc, off);
-		const int o_pos = __shfl_xor_sync(FULL, pos, off), o_row = __shfl_xor_sync(FULL, row, off);
-		if (o_sc > sc || (o_sc == sc && (o_pos < pos || (o_pos == pos && o_row < row)))) { sc = o_sc; pos = o_pos; row = o_row; }
-	}
-	if (sc == 0) { pos = 0; row = 0; }
-	const bool unarmed = sc > 0 && pos < 0;          /* the maximum lies before the armed range of its item: no position, no row */
-	if (unarmed) { pos = 0; row = 0; }
+	const SswItemBest bc = best[idx];
+	int sc = bc.score[h], pos = bc.pos[h], row = bc.row[h];
+	if (sc <= 0) { sc = 0; pos = 0; row = 0; }
 
 	SswFillResult r;
 	r.score = sc; r.ref = pos; r.read = row < d.read_len - 1 ? row : d.read_len - 1;
 	r.score2 = 0; r.ref2 = 0; r.overflow = 0; r.pad_[0] = r.pad_[1] = 0;
 	if (sc == 0) { r.ref = d.word ? 0 : -1; r.read = 0; }
 	if (sc >= d.limit) { r.overflow = d.word ? 2 : 1; if (!d.word) r.score = 255; }
-	else if (unarmed) r.overflow = 3;                 /* the caller re-does the pair with arm 0 */
 
 	int slots[SSW_REFILL_SLOTS] = {-1, -1, -1, -1};     /* block ids; the zone slot: its first column */
 	int zone_end = 0;
@@ -174,64 +205,41 @@ ssw_resolve_blocks_kernel(const SswAlnDesc* __restrict__ alns, int n_aln,
 		const int e1 = max(pos - d.mask_len, 0);
 		const int e2 = min(pos + d.mask_len, d.ref_len) + (d.word ? 0 : 1);
 		if (d.byte_pad > 0 && e2 < d.ref_len) { slots[SSW_REFILL_ZONE] = e2 & ~3; zone_end = min(e2 + 8, d.ref_len); }
+		/* every fully allowed block is a candidate (value, block); chunks start at block boundaries, so the blocks of the
+		 * pair-task's row are those of its items */
 		const uint32_t* bm = blkmax + d.cm_off;
-		int vx = 0, ix = 0;                  /* best exact candidate: items that do not touch the window */
-		int vb = 0, bb = 0x7fffffff;         /* best fully allowed block of the items that do: (value, smallest block) */
-		for (int k0 = 0; k0 < d.n_items; k0 += 32) {
-			const int k = k0 + lane;
-			bool straddles = false;
-			int p0 = 0, p1 = 0;
-			if (k < d.n_items) {
-				const SswItemBest b = bests[d.first_item + k];
-				p0 = b.p0; p1 = b.p1;
-				if (p1 <= e1 || p0 >= e2) { if (ssw_second_better(b.score[h], b.pos[h], vx, ix)) { vx = b.score[h]; ix = b.pos[h]; } }
-				else straddles = p1 > p0;
-			}
-			unsigned todo = __ballot_sync(FULL, straddles);
-			while (todo) {
-				const int src = __ffs((int)todo) - 1;
-				todo &= todo - 1;
-				const int q0 = __shfl_sync(FULL, p0, src), q1 = __shfl_sync(FULL, p1, src);
-				for (int b = q0 / SSW_CM_BLOCK + lane; b * SSW_CM_BLOCK < q1; b += 32) {
-					const int bs = b * SSW_CM_BLOCK, be = min(bs + SSW_CM_BLOCK, q1);
-					if (be <= e1 || bs >= e2) {
-						const int v = half_of(bm[b], h);
-						if (v > vb || (v == vb && v > 0 && b < bb)) { vb = v; bb = b; }
-					}
-				}
+		const int n_blk = (d.ref_len + SSW_CM_BLOCK - 1) / SSW_CM_BLOCK;
+		int vb = 0, bb = 0x7fffffff;
+		for (int b = lane; b < n_blk; b += 32) {
+			const int bs = b * SSW_CM_BLOCK, be = min(bs + SSW_CM_BLOCK, d.ref_len);
+			if (be <= e1 || bs >= e2) {
+				const int v = half_of(bm[b], h);
+				if (v > vb) { vb = v; bb = b; }
 			}
 		}
 #pragma unroll
 		for (int off = 16; off >= 1; off >>= 1) {
-			const int o_v = __shfl_xor_sync(FULL, vx, off), o_i = __shfl_xor_sync(FULL, ix, off);
-			if (ssw_second_better(o_v, o_i, vx, ix)) { vx = o_v; ix = o_i; }
 			const int o_vb = __shfl_xor_sync(FULL, vb, off), o_bb = __shfl_xor_sync(FULL, bb, off);
 			if (o_vb > vb || (o_vb == vb && o_vb > 0 && o_bb < bb)) { vb = o_vb; bb = o_bb; }
 		}
-		r.score2 = vx; r.ref2 = ix;
 		/* blocks cut by the window edges (e1 > 0 and e2 < ref_len whenever the remainder is non-zero / tested) */
 		if (e1 % SSW_CM_BLOCK) slots[0] = e1 / SSW_CM_BLOCK;
 		if ((e2 % SSW_CM_BLOCK) && e2 < d.ref_len && e2 / SSW_CM_BLOCK != slots[0]) slots[1] = e2 / SSW_CM_BLOCK;
-		if (vb > 0 && vb >= vx) slots[2] = bb;
+		if (vb > 0) slots[2] = bb;
 	}
 	if (lane == 0) out[idx] = r;
 	if (lane < SSW_REFILL_SLOTS) {
 		const int b = slots[lane];
 		const int64_t slot = (int64_t)idx * SSW_REFILL_SLOTS + lane;
-		SswItem it = items[d.n_items > 0 ? d.first_item : 0];
-		it.term_a = -1; it.cend = 0;
-		int c0 = -1;
-		if (b >= 0) {
-			if (lane == SSW_REFILL_ZONE) {
-				it.p0 = b; it.p1 = zone_end;
-				if (h) it.qb.lp += d.byte_pad; else it.qa.lp += d.byte_pad;
-			} else { it.p0 = b * SSW_CM_BLOCK; it.p1 = min(it.p0 + SSW_CM_BLOCK, d.ref_len); }
-			it.warm = min(d.warm, it.p0);     /* d.warm is taken from the byte padding */
-			it.cm_off = slot * SSW_CM_BLOCK - it.p0;
-			c0 = it.p0;
-		} else { it.p0 = it.p1 = 0; it.warm = 0; it.cm_off = SSW_CM_NONE; }
+		SswItem it;
+		if (b < 0) it = ssw_refill_item(d, items, 0, 0);
+		else if (lane == SSW_REFILL_ZONE) {
+			it = ssw_refill_item(d, items, b, zone_end);
+			if (h) it.qb.lp += d.byte_pad; else it.qa.lp += d.byte_pad;
+		} else it = ssw_refill_item(d, items, b * SSW_CM_BLOCK, min(b * SSW_CM_BLOCK + SSW_CM_BLOCK, d.ref_len));
+		if (b >= 0) it.cm_off = slot * SSW_CM_BLOCK - it.p0;
 		refill_items[slot] = it;
-		refill_c0[slot] = c0;
+		refill_c0[slot] = b >= 0 ? it.p0 : -1;
 	}
 }
 
