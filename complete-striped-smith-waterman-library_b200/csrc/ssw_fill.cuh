@@ -8,6 +8,7 @@
  *     H(c,r) = max(X(c,r), F(c,r))
  *     E(c+1,r) = max(E(c,r) - gapE, X(c,r) - gapO)
  *     F(c,r+1) = max(F(c,r) - gapE, X(c,r) - gapO)          (gapO > gapE)
+ * (block mode computes the same H and F with the gap openings taken from H, as ssw.c does: ssw_cells)
  * in wrap-free signed 16-bit arithmetic, two alignments per register (s16x2
  * DPX instructions: VIADDMNMX.S16x2[.RELU], VIMNMX[3].S16x2, VIADD.16x2).
  * No lazy-F loop exists here: F is carried exactly down the column.
@@ -157,11 +158,23 @@ __device__ static __forceinline__ void ssw_load_scores(uint32_t (&s)[R], ssw_sad
 	}
 }
 
-/* The R cells of one lane in one column: 5 DPX/ALU instructions per cell pair + 1/2 for the column maximum.
+/* The R cells of one lane in one column, + 1/2 ALU instruction per cell pair for the column maximum.
  * In: Hd (H of the previous column, shifted down one row), E, scores, and (inH, inF) from the lane above.
  * Out: Hn (H of this column), updated E and Hd, outH/outF/outC for the lane below (outC = maximum of the column
- * over the rows of this lane and of all lanes above it). */
-template <int R>
+ * over the rows of this lane and of all lanes above it).
+ *
+ * Two forms of the cell, selected by FROM_H:
+ *   false  X = max(Hd + s, E, 0), H = max(X, F), E' = max(E - gapE, X - gapO), F' = max(F - gapE, X - gapO):
+ *          VIADDMNMX.RELU, VIADD.16x2, VIADDMNMX x2, VIMNMX -- 4 ALU-pipe instructions + 1 packed add per cell pair
+ *   true   H = max(Hd + s, E, F, 0), E' = max(E - gapE, H - gapO), F' = max(F - gapE, H - gapO) (ssw.c's form):
+ *          VIADD.16x2 x2, VIMNMX3.RELU, VIADDMNMX x2 -- 3 ALU-pipe instructions + 2 packed adds, which do not issue
+ *          on the ALU pipe (DESIGN 4.1, tools/microbench.cu)
+ * Both give the same H and F in every cell (so the same outH, outF, outC and column maxima); only E differs, by the term
+ * F - gapO, and E never leaves the lane.  With gapO > gapE: H - gapO = max(X - gapO, F - gapO) and F - gapO < F - gapE,
+ * so F' is the same; E of the second form also admits a horizontal gap right after a vertical one (F -> E), and any
+ * such path has a companion of no lower score that takes the same moves horizontal first, which the first form admits
+ * (E -> F through X), so H is the same.  tests/test_cell_form.py checks both forms against the oracle and each other. */
+template <int R, bool FROM_H>
 __device__ static __forceinline__ void ssw_cells(uint32_t (&Hd)[R], uint32_t (&E)[R], const uint32_t (&s)[R], uint32_t (&Hn)[R],
                                                 uint32_t inH, uint32_t inF, uint32_t inC, uint32_t negO, uint32_t negE,
                                                 uint32_t& outH, uint32_t& outF, uint32_t& outC, uint32_t& own)
@@ -169,11 +182,21 @@ __device__ static __forceinline__ void ssw_cells(uint32_t (&Hd)[R], uint32_t (&E
 	uint32_t F = inF;
 #pragma unroll
 	for (int k = 0; k < R; ++k) {
-		const uint32_t X = __viaddmax_s16x2_relu(Hd[k], s[k], E[k]);
-		const uint32_t Xg = __vadd2(X, negO);
-		E[k] = __viaddmax_s16x2(E[k], negE, Xg);
-		Hn[k] = __vmaxs2(X, F);
-		F = __viaddmax_s16x2(F, negE, Xg);
+		if constexpr (FROM_H) {
+			/* The sum goes in as the LAST operand of the three-way maximum: given as the first, ptxas fuses it into a
+			 * VIADDMNMX.RELU with E and adds a VIMNMX.RELU for F, which is the first form's ALU count again. */
+			const uint32_t T = __vadd2(Hd[k], s[k]);
+			Hn[k] = __vimax3_s16x2_relu(E[k], F, T);
+			const uint32_t Hg = __vadd2(Hn[k], negO);
+			E[k] = __viaddmax_s16x2(E[k], negE, Hg);
+			F = __viaddmax_s16x2(F, negE, Hg);
+		} else {
+			const uint32_t X = __viaddmax_s16x2_relu(Hd[k], s[k], E[k]);
+			const uint32_t Xg = __vadd2(X, negO);
+			E[k] = __viaddmax_s16x2(E[k], negE, Xg);
+			Hn[k] = __vmaxs2(X, F);
+			F = __viaddmax_s16x2(F, negE, Xg);
+		}
 	}
 	/* `own`: maximum of the column over this lane's rows (the best-cell bookkeeping compares it with the lane's running
 	 * best); outC: the partial column maximum handed down the lanes, own folded with the value from above */
@@ -398,8 +421,15 @@ ssw_fill_kernel(const SswItem* __restrict__ items, int n_items,
 	int sL = (it.p0 - it.warm - (G - 1)) & (CM == 2 ? ~7 : ~3);   /* scan position of the group's last lane, multiple of 4 (block mode: of 8) */
 	constexpr int U = 8;                                /* scan positions per loop body */
 	int n_body = live && it.p1 > sL ? (it.p1 - sL + U - 1) / U : 0;
-#pragma unroll
+	/* the longest group's count, in a uniform register (REDUX): the loop branch is then uniform, and ptxas issues the
+	 * shuffles of the step without the per-step WARPSYNC.COLLECTIVE guards and register copies of a loop it cannot
+	 * prove warp-uniform (about 120 instructions per loop body of the (8,19) instance).  The emulator build takes the
+	 * same maximum with a shuffle butterfly. */
+#ifdef SSW_CPU_EMU
 	for (int off = G; off < 32; off <<= 1) n_body = max(n_body, __shfl_xor_sync(FULL, n_body, off));
+#else
+	n_body = __reduce_max_sync(FULL, n_body);
+#endif
 
 	/* column cursor of this lane for step j = 0 of the current body, clamped into the padded array */
 	int col = DIR > 0 ? sL + (G - 1 - t) : it.cend - (sL + (G - 1 - t));
@@ -423,6 +453,9 @@ ssw_fill_kernel(const SswItem* __restrict__ items, int n_items,
 	/* Block mode keeps no best cell: the resolve takes the score and the first block holding it from the block maxima and
 	 * re-fills that one block with tracking (ssw_resolve.cuh).  So its sweep carries only the recurrence and the maxima. */
 	constexpr bool TRACK = CM != 2;
+	/* Block mode computes the cells in the form with 3 ALU-pipe instructions per cell pair (ssw_cells); the other instances
+	 * keep the 4-instruction form, since the 3-instruction form has been timed only in block mode (configs 2 and 3). */
+	constexpr bool FROM_H = CM == 2;
 	SswLaneBest lb;
 	lb.best = 0; lb.pos0 = lb.pos1 = -1; lb.row0 = lb.row1 = 0;      /* position -1: no recorded event (yet) */
 	SswSnap<R> snap;
@@ -457,7 +490,7 @@ ssw_fill_kernel(const SswItem* __restrict__ items, int n_items,
 			uint32_t s[R], Hn[R];
 			ssw_load_scores<R>(s, pbase, ptail, letter);
 			uint32_t own;
-			ssw_cells<R>(Hd, E, s, Hn, inH, inF, inC, negO, negE, outH, outF, outC, own);
+			ssw_cells<R, FROM_H>(Hd, E, s, Hn, inH, inF, inC, negO, negE, outH, outF, outC, own);
 			cmv[j] = outC;
 
 			/* running best of this lane's rows (strict increase only; rare path) */
@@ -755,7 +788,7 @@ ssw_fill_strips_kernel(const SswStripTask* __restrict__ tasks,
 							for (int k = 0; k < R; ++k) sc[k] = (sc[k] & 0x0000ffffu) | (sb[k] & 0xffff0000u);
 						}
 						uint32_t own;
-						ssw_cells<R>(Hd, E, sc, Hn, inH, inF, inC, negO, negE, outH, outF, outC, own);
+						ssw_cells<R, false>(Hd, E, sc, Hn, inH, inF, inC, negO, negE, outH, outF, outC, own);
 						cmv[j] = outC; hv[j] = outH; fv[j] = outF;
 						const uint32_t nb = __vmaxs2(lb.best, own);
 						if (nb != lb.best && maybe_counted) ssw_track<R>(lb, snap, nb, Hn, sp0 + 4 * h + j, 0, T.p1);

@@ -155,6 +155,38 @@ __global__ void probe_pipes(uint32_t* out, long long* cyc, uint32_t seed)
 	if (threadIdx.x == 0) cyc[blockIdx.x] = t1 - t0;
 }
 
+// NA VIADDMNMX.S16x2 and NB VIADD.16x2 (packed 16-bit add, no maximum) per inner step, every chain independent: does the
+// packed add issue on the ALU pipe beside the DPX instructions, or on another one?
+template <int NA, int NB>
+__global__ void probe_mix_viadd(uint32_t* out, long long* cyc, uint32_t seed)
+{
+	uint32_t va[8], vb[8];
+#pragma unroll
+	for (int i = 0; i < 8; ++i) { va[i] = seed * (i + 1) + threadIdx.x; vb[i] = seed * (i + 9) + threadIdx.x; }
+	uint32_t b = (seed & 0x00030003u) | 0x00010001u, c = 0xfffcfffcu, d = seed | 0x00010001u;
+	asm volatile("" : "+r"(b), "+r"(c), "+r"(d));
+	__syncthreads();
+	long long t0 = clock64();
+#pragma unroll 1
+	for (int it = 0; it < ITERS; ++it) {
+#pragma unroll
+		for (int u = 0; u < 4; ++u) {
+#pragma unroll
+			for (int i = 0; i < (NA > NB ? NA : NB); ++i) {
+				if (i < NA) va[i] = __viaddmax_s16x2(va[i], b, c);
+				if (i < NB) vb[i] = __vadd2(vb[i], (u & 1) ? d : b);   // alternating addends: no chain of equal adds to fold
+			}
+		}
+		d ^= (uint32_t)it;
+	}
+	long long t1 = clock64();
+	uint32_t acc = 0;
+#pragma unroll
+	for (int i = 0; i < 8; ++i) acc ^= va[i] ^ vb[i];
+	out[blockIdx.x * blockDim.x + threadIdx.x] = acc;
+	if (threadIdx.x == 0) cyc[blockIdx.x] = t1 - t0;
+}
+
 // The recurrence itself, R rows per lane, no memory traffic: scores rotate through registers.
 //   MODE 0: the shipped s16x2 formulation (5 ALU-pipe DPX ops per cell pair)
 //   MODE 1: packed-half formulation: 4 HFMA2.RELU (FMA pipe) + 4 VIMNMX.S16x2 (ALU pipe) per cell pair; all values >= 0 so the
@@ -234,23 +266,28 @@ __global__ void probe_cells(uint32_t* out, long long* cyc, uint32_t seed)
 //   FORM 1: biased values (every stored value >= 0, so a packed 16x2 add is an exact 32-bit add): Hd+s and X-gapO as IMAD on the
 //           FMA pipe, X = VIMNMX3(t, E, floor), E'/F' = VIADDMNMX, H = VIMNMX: 4 ALU + 2 FMA per cell pair
 //   FORM 2: biased values, all four adds as IMAD, four maxima on the ALU pipe: 4 ALU + 4 FMA per cell pair
+//   FORM 3: ssw.c's form, as the block-mode fill computes it (ssw_cells<R, true>): T = Hd + s and H - gapO as VIADD.16x2,
+//           H = VIMNMX3.RELU(E, F, T), E'/F' = VIADDMNMX: 3 ALU + 2 VIADD.16x2 per cell pair
+// Rows per lane that are not a multiple of 4 are stored like the fill kernel stores R = 19: a full last segment, unused words.
 template <int R, int FORM>
 __global__ void probe_body(uint32_t* out, long long* cyc, uint32_t seed)
 {
-	__shared__ __align__(16) uint32_t prof[4 * 32 * R];
+	constexpr int S = (R + 3) / 4 * 4;
+	__shared__ __align__(16) uint32_t prof[4 * 32 * S];
 	const int lane = threadIdx.x & 31;
-	for (int i = threadIdx.x; i < 4 * 32 * R; i += blockDim.x) {
+	for (int i = threadIdx.x; i < 4 * 32 * S; i += blockDim.x) {
 		const int v = (int)((seed * (i + 3)) % 5) - 2;
 		uint32_t w = ((uint32_t)v & 0xffffu) | ((uint32_t)v << 16);
-		if (FORM != 0 && v < 0) w -= 0x10000u;           // carry compensation of the packed 32-bit add
+		if ((FORM == 1 || FORM == 2) && v < 0) w -= 0x10000u;   // carry compensation of the packed 32-bit add
 		prof[i] = w;
 	}
 	__syncthreads();
-	const uint32_t B = FORM == 0 ? 0u : 0x02000200u;      // bias 512 per half
+	const bool biased = FORM == 1 || FORM == 2;
+	const uint32_t B = biased ? 0x02000200u : 0u;         // bias 512 per half
 	uint32_t Hd[R], E[R];
 #pragma unroll
 	for (int k = 0; k < R; ++k) { Hd[k] = B; E[k] = B; }
-	uint32_t negO = FORM == 0 ? 0xfffdfffdu : (uint32_t)(-(int)(3u * 0x10001u));
+	uint32_t negO = !biased ? 0xfffdfffdu : (uint32_t)(-(int)(3u * 0x10001u));
 	uint32_t negE = 0xffffffffu;                          // -1 | -1 (VIADDMNMX operand)
 	uint32_t negE32 = (uint32_t)(-(int)(0x10001u));
 	uint32_t one = seed - 12344u /* == 1 at run time, unknown to the compiler: keeps the packed adds IMADs */, keep = lane == 0 ? 0u : 1u, floorB = B, top_add = lane == 0 ? B : 0u;
@@ -268,13 +305,21 @@ __global__ void probe_body(uint32_t* out, long long* cyc, uint32_t seed)
 			const int letter = (it + u + (int)(best & 1u)) & 3;
 			uint32_t s[R], Hn[R];
 #pragma unroll
-			for (int q = 0; q < R / 4; ++q) {
-				const uint4 v = *reinterpret_cast<const uint4*>(&prof[letter * 32 * R + q * 128 + lane * 4]);
-				s[4 * q] = v.x; s[4 * q + 1] = v.y; s[4 * q + 2] = v.z; s[4 * q + 3] = v.w;
+			for (int q = 0; q < S / 4; ++q) {
+				const uint4 v = *reinterpret_cast<const uint4*>(&prof[letter * 32 * S + q * 128 + lane * 4]);
+				const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+				for (int j = 0; j < 4; ++j) if (4 * q + j < R) s[4 * q + j] = w[j];
 			}
 #pragma unroll
 			for (int k = 0; k < R; ++k) {
-				if (FORM == 0) {
+				if (FORM == 3) {
+					const uint32_t t = __vadd2(Hd[k], s[k]);
+					Hn[k] = __vimax3_s16x2_relu(E[k], F, t);
+					const uint32_t Hg = __vadd2(Hn[k], negO);
+					E[k] = __viaddmax_s16x2(E[k], negE, Hg);
+					F = __viaddmax_s16x2(F, negE, Hg);
+				} else if (FORM == 0) {
 					const uint32_t X = __viaddmax_s16x2_relu(Hd[k], s[k], E[k]);
 					const uint32_t Xg = __vadd2(X, negO);
 					E[k] = __viaddmax_s16x2(E[k], negE, Xg);
@@ -474,6 +519,11 @@ int main()
 			const double h08 = run(probe<9>, threads, 4 * ILP, sms);
 			printf(", \"mix_dpx_hmnmx2_1024thr\": {\"8+0\": %.3f, \"6+2\": %.3f, \"4+4\": %.3f, \"HMNMX2 alone\": %.3f}", h80, h62, h44, h08);
 			printf(", \"mix_dpx_imad_1024thr\": {\"4+4\": %.3f, \"6+2\": %.3f, \"8+0\": %.3f}", m44, m62, m80);
+			// VIADDMNMX + VIADD.16x2 per unit: the issue rate of both together (warp-instructions per clock per SM); 0+8 = VIADD.16x2 alone
+			printf(", \"mix_dpx_viadd_1024thr\": {\"8+0\": %.3f, \"6+2\": %.3f, \"4+4\": %.3f, \"3+2\": %.3f, \"0+8\": %.3f}",
+			       run(probe_mix_viadd<8, 0>, threads, 4 * 8, sms), run(probe_mix_viadd<6, 2>, threads, 4 * 8, sms),
+			       run(probe_mix_viadd<4, 4>, threads, 4 * 8, sms), run(probe_mix_viadd<3, 2>, threads, 4 * 5, sms),
+			       run(probe_mix_viadd<0, 8>, threads, 4 * 8, sms));
 			// fill kernel: 5.5 DPX ops per lane per two cells -> cells/clk/SM = rate * 32 lanes * 2 / 5.5
 
 			// round 2: second-pipe probes
@@ -502,7 +552,13 @@ int main()
 			for (int thr = 256; thr <= 512; thr *= 2) {
 				const double k = 32.0 * 2.0 * 20.0 * sms * (clk_khz * 1e3) / 1e9;
 				const double b0 = run(probe_body<20, 0>, thr, 1, sms), b1 = run(probe_body<20, 1>, thr, 1, sms), b2 = run(probe_body<20, 2>, thr, 1, sms);
-				printf(", \"fill_body_R20_%dthr_gcups\": {\"shipped: 5 ALU per cell pair\": %.1f, \"biased: 4 ALU + 2 IMAD\": %.1f, \"biased: 4 ALU + 4 IMAD\": %.1f}", thr, b0 * k, b1 * k, b2 * k);
+				const double b3 = run(probe_body<20, 3>, thr, 1, sms);
+				printf(", \"fill_body_R20_%dthr_gcups\": {\"shipped: 5 ALU per cell pair\": %.1f, \"biased: 4 ALU + 2 IMAD\": %.1f, \"biased: 4 ALU + 4 IMAD\": %.1f, \"3 ALU + 2 VIADD.16x2\": %.1f}", thr, b0 * k, b1 * k, b2 * k, b3 * k);
+			}
+			for (int thr = 256; thr <= 512; thr *= 2) {
+				const double k = 32.0 * 2.0 * 19.0 * sms * (clk_khz * 1e3) / 1e9;
+				printf(", \"fill_body_R19_%dthr_gcups\": {\"shipped: 4 ALU + 1 VIADD.16x2\": %.1f, \"3 ALU + 2 VIADD.16x2\": %.1f}", thr,
+				       run(probe_body<19, 0>, thr, 1, sms) * k, run(probe_body<19, 3>, thr, 1, sms) * k);
 			}
 			{
 				const double k = 32.0 * 2.0 * 20.0 * sms * (clk_khz * 1e3) / 1e9;
