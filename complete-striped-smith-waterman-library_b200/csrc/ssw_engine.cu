@@ -185,6 +185,7 @@ struct ssw_engine {
 	SswDevBuf d_hits;                                        /* ssw_engine_search: the n_q x k hit table of the grid path */
 	SswDevBuf d_mark;                                        /* ssw_engine_mark_mismatch: tasks, input CIGARs, marked CIGARs */
 	SswDevBuf d_rf_items, d_rf_bests, d_rf_blk, d_rf_cm;     /* block-maximum mode: re-fill items, their (unused) bests, first columns, column maxima */
+	int64_t last_cm_words = 0;                               /* column-maximum words of the last forward launch (ssw_engine_last_colmax) */
 	SswStagedD2H staged;
 	cudaStream_t side[3] = {nullptr, nullptr, nullptr};     /* traceback launches of different kernel shapes run side by side */
 	ssw_engine* kids[SSW_MAX_SLICES] = {};                  /* helper engines of the sliced path (views of this engine's sequences) */
@@ -387,6 +388,17 @@ extern "C" int ssw_engine_last_timing(const ssw_engine* e, ssw_engine_timing* t)
 	if (!e || !t) return -1;
 	*t = e->timing;
 	return 0;
+}
+
+extern "C" int64_t ssw_engine_last_colmax(ssw_engine* e, uint32_t* out, int64_t n_words)
+{
+	if (!e || n_words < 0 || (n_words > 0 && !out)) return -1;
+	const int64_t n = std::min(n_words, e->last_cm_words);
+	if (n > 0) {
+		SSW_CUDA_OK(cudaStreamSynchronize(e->stream));
+		SSW_CUDA_OK(cudaMemcpy(out, e->d_colmax.p, sizeof(uint32_t) * (size_t)n, cudaMemcpyDeviceToHost));
+	}
+	return e->last_cm_words;
 }
 
 /* References are stored as  [PAD x null] codes [PAD x null]  with null = n (scores as a dead letter), each block
@@ -1159,10 +1171,13 @@ static int forward_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Al
 				while (items.size() % (size_t)per_cta) items.push_back(dead);
 			}
 			const int first_item = (int)items.size();
+			/* block mode: every item starts its sweep (p0 - warm) at a block boundary, which the block-mode fill relies on to
+			 * find the blocks of all its lanes from the loop count alone (ssw_fill.cuh); a longer warm-up is just as exact */
+			const int32_t warm = block ? (pl.warm + SSW_CM_BLOCK - 1) / SSW_CM_BLOCK * SSW_CM_BLOCK : pl.warm;
 			for (int c = 0; c < pl.n_chunks; ++c) {
 				it.p0 = (int32_t)((int64_t)c * pl.chunk);
 				it.p1 = (int32_t)std::min<int64_t>(ref_len, (int64_t)(c + 1) * pl.chunk);
-				it.warm = std::min(pl.warm, it.p0);
+				it.warm = std::min(warm, it.p0);
 				it.cm_off = (int64_t)cm_words;
 				items.push_back(it);
 				cells += (int64_t)(it.p1 - it.p0 + it.warm) * inst_rows(inst) * 2;
@@ -1184,6 +1199,7 @@ static int forward_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Al
 		tr.lap("forward: plan");
 		if (e->d_colmax.ensure(cm_words * 4 + 64)) return -1;
 		if (e->run_fill(items, inst, +1, block ? 2 : 1, share, P, &e->timing.fill_forward_ms)) return -1;
+		e->last_cm_words = (int64_t)cm_words;
 		tr.lap("forward: fill (copy+kernel)");
 		e->timing.fill_forward_launches += 1;
 		e->timing.cells_forward += cells;

@@ -17,7 +17,7 @@
  * [t*R, t*R+R).  The group sweeps the reference as a skewed wavefront: in one
  * step lane t works on scan position s - t, so that the three values that
  * cross a lane boundary (bottom H, outgoing F, partial column maximum) are
- * handed down with one __shfl_up each.  Per-letter query profiles (both
+ * handed down with one __shfl_up each (block mode: H and F only).  Per-letter query profiles (both
  * alignments packed) live in shared memory; reference letters stream from
  * the padded reference array (null letters outside [0, refLen) keep the state
  * at exactly zero, so pipeline fill and drain need no predication).
@@ -369,7 +369,8 @@ __device__ static __forceinline__ void ssw_reduce_best(const SswLaneBest& lb, in
  *   2  one packed word per block of SSW_CM_BLOCK columns, and no best cell (`bests` is not written).  The best cell needs
  *      single columns only in the first block holding the largest block maximum, the second-best scan (ssw.c:368-381) only
  *      in the <= 2 blocks cut by the mask window and in the block that holds the winner; ssw_resolve.cuh re-fills those
- *      blocks per alignment with mode 1.  Chunks start at multiples of SSW_CM_BLOCK. */
+ *      blocks per alignment with mode 1.  Chunks start at multiples of SSW_CM_BLOCK, and so does every item's sweep
+ *      (p0 - warm: the planner rounds the warm-up up to a multiple of SSW_CM_BLOCK). */
 /* WARPS: warps per CTA.  4 by default; 8 where one CTA-shared profile is so large (protein alphabets: 64 KB at 20 rows per
  * lane) that four-warp CTAs would leave the SM with 8 resident warps -- eight warps per profile keep 16. */
 /* ARM: items may carry a late arming position (SswItem.cend, device-planned grids); a template parameter so that the kernels
@@ -420,7 +421,10 @@ ssw_fill_kernel(const SswItem* __restrict__ items, int n_items,
 	const uint32_t negO = pack2(-gapO, -gapO), negE = pack2(-gapE, -gapE);
 	int sL = (it.p0 - it.warm - (G - 1)) & (CM == 2 ? ~7 : ~3);   /* scan position of the group's last lane, multiple of 4 (block mode: of 8) */
 	constexpr int U = 8;                                /* scan positions per loop body */
-	int n_body = live && it.p1 > sL ? (it.p1 - sL + U - 1) / U : 0;
+	/* block mode sweeps on to the end of the last block, so that its last lane finishes that block inside the loop (the
+	 * columns behind the reference leave the block maximum as it is, see the block fold below) */
+	const int p_end = CM == 2 ? (it.p1 + SSW_CM_BLOCK - 1) & ~(SSW_CM_BLOCK - 1) : it.p1;
+	int n_body = live && it.p1 > sL ? (p_end - sL + U - 1) / U : 0;
 	/* the longest group's count, in a uniform register (REDUX): the loop branch is then uniform, and ptxas issues the
 	 * shuffles of the step without the per-step WARPSYNC.COLLECTIVE guards and register copies of a loop it cannot
 	 * prove warp-uniform (about 120 instructions per loop body of the (8,19) instance).  The emulator build takes the
@@ -440,11 +444,11 @@ ssw_fill_kernel(const SswItem* __restrict__ items, int n_items,
 	/* per-lane shared-memory cursors: rows 0..4*A4-1 as uint4 segments, the tail behind them */
 	const ssw_saddr pbase = ssw_sadd(ssw_sbase(prof), lane * 4);
 	const ssw_saddr ptail = ssw_sadd(ssw_sbase(prof), A4 * 128 + lane * REM);
-	uint32_t top_keep = t == 0 ? 0u : 1u;               /* lane 0 of a group takes zeros from above (multiplied in: FMA pipe) */
+	/* Lane 0 of a group takes zeros from above (multiplied in: FMA pipe).  The 0/1 is fetched from the lane before with a
+	 * shuffle, which ptxas keeps in a register; derived from the thread index, ptxas rebuilds it inside the loop (S2R, LOP3,
+	 * ISETP, SEL).  Being opaque to the compiler, it also keeps the masking a multiply. */
+	const uint32_t top_keep = __shfl_sync(FULL, t == G - 1 ? 0u : 1u, t + G - 1, G);
 	const uint8_t* lptr = rp + col;                     /* letter cursor, advanced together with col */
-#ifndef SSW_CPU_EMU
-	asm volatile("" : "+r"(top_keep) : : "memory");     /* opaque 0/1 so that the masking stays a multiply */
-#endif
 
 	uint32_t Hd[R], E[R];
 #pragma unroll
@@ -461,10 +465,10 @@ ssw_fill_kernel(const SswItem* __restrict__ items, int n_items,
 	SswSnap<R> snap;
 	if constexpr (TRACK)
 		ssw_snap_init<R>(snap, reinterpret_cast<uint4*>(smem + (size_t)(share ? 1 : nwarps) * (size_t)(n + 1) * 32 * S), (int)threadIdx.x);
-	uint32_t blk_acc = 0;                               /* CM == 2: running maximum of the current block (last lane) */
+	uint32_t blk_acc = 0, blk_done = 0;                 /* CM == 2: this lane's maximum of its current block, and of its last finished one */
 
 	for (int body = 0; body < n_body; ++body) {
-		uint32_t cmv[U];
+		uint32_t cmv[U];                                /* per step: outC, or in block mode the maximum over this lane's own rows */
 		if (TRACK && (body & (SSW_FLOOR_PERIOD - 1)) == 0) {
 			/* lower bound of the group's final maximum: a lane value below it can never be the best cell, so the lane's
 			 * running best is raised to (bound - 1) and such values no longer trigger the bookkeeping */
@@ -482,7 +486,7 @@ ssw_fill_kernel(const SswItem* __restrict__ items, int n_items,
 			/* values crossing the lane boundary */
 			const uint32_t inH = __shfl_up_sync(FULL, outH, 1, G) * top_keep;
 			const uint32_t inF = __shfl_up_sync(FULL, outF, 1, G) * top_keep;
-			const uint32_t inC = __shfl_up_sync(FULL, outC, 1, G) * top_keep;
+			const uint32_t inC = CM == 2 ? 0u : __shfl_up_sync(FULL, outC, 1, G) * top_keep;   /* block mode: outC unused */
 
 			/* reference letter of this lane's scan position and its profile rows */
 			int letter = (int)lptr[DIR * j];
@@ -491,7 +495,7 @@ ssw_fill_kernel(const SswItem* __restrict__ items, int n_items,
 			ssw_load_scores<R>(s, pbase, ptail, letter);
 			uint32_t own;
 			ssw_cells<R, FROM_H>(Hd, E, s, Hn, inH, inF, inC, negO, negE, outH, outF, outC, own);
-			cmv[j] = outC;
+			cmv[j] = CM == 2 ? own : outC;
 
 			/* running best of this lane's rows (strict increase only; rare path) */
 			if constexpr (TRACK) {
@@ -513,20 +517,39 @@ ssw_fill_kernel(const SswItem* __restrict__ items, int n_items,
 			}
 		}
 		if (CM == 2) {
-			/* p0 and sL are multiples of 8 here, so a body lies entirely before p0 or not at all; only the last body of the
-			 * reference can be cut by p1 (chunks end at block boundaries).  Its columns behind the reference are folded in as
-			 * well: there the null letters leave X = max(0, E) with E(c) <= H(c-1) of the same row, and F only carries X down,
-			 * so such a column's maximum never exceeds that of the column before it -- the block maximum stays the same, and
-			 * the body needs no per-column predicates (which would be issued on every body). */
-			if (t == G - 1 && it.cm_off != SSW_CM_NONE && sL >= it.p0 && sL < it.p1) {
+			/* Block maxima per lane.  A block maximum is the maximum over all cells of the block, so every lane keeps its own
+			 * over the cells of its rows, and the group combines the lanes once per block: no column maximum travels down the
+			 * lanes.  The planner starts every block-mode item at a multiple of SSW_CM_BLOCK (p0 - warm), so sL = p0 - warm - G
+			 * at body 0 and lane t is at column 8 * body + j - 1 - t (mod 64) in step j: its next block starts at step
+			 * js = t + 1 - 8 * (body mod 8) of a body with body mod 8 < G / 8 (js = 8: right after it), and the last lane
+			 * finishes a block at the end of the body with body mod 8 = G / 8 - 1, when every lane of the group has finished
+			 * it (a lane is at most G - 1 <= 31 columns ahead, so it holds at most one finished block).  These tests are on
+			 * `body`, which is warp-uniform: the bodies between carry no per-step predicate.  The columns behind the reference
+			 * are folded in as well: there the null letters leave X = max(0, E) with E(c) <= H(c-1) of the same row, and F
+			 * only carries X down, so such a column's maximum never exceeds that of the column before it, and the block
+			 * maximum stays the same.  Columns before p0 or of the next chunk end up only in blocks that are not stored. */
+			constexpr int BODIES = SSW_CM_BLOCK / U;            /* loop bodies per block */
+			const int bm = body % BODIES;
+			if (bm < G / U) {
+				const int js = t + 1 - U * bm;
+				uint32_t lo = blk_acc, hi = 0;
+#pragma unroll
+				for (int j = 0; j < U; ++j) {
+					if (j < js) lo = __vmaxs2(lo, cmv[j]);
+					else hi = __vmaxs2(hi, cmv[j]);
+				}
+				if (js >= 1 && js <= U) { blk_done = lo; blk_acc = hi; }
+				else blk_acc = __vmaxs2(lo, hi);
+				if (bm == G / U - 1) {
+					const uint32_t v = ssw_group_max<G>(blk_done);
+					const int c0 = sL + U - SSW_CM_BLOCK;       /* first column of the block just finished */
+					if (t == 0 && it.cm_off != SSW_CM_NONE && c0 >= it.p0 && c0 < it.p1) colmax[it.cm_off + c0 / SSW_CM_BLOCK] = v;
+				}
+			} else {
 				blk_acc = __vimax3_s16x2(blk_acc, cmv[0], cmv[1]);
 				blk_acc = __vimax3_s16x2(blk_acc, cmv[2], cmv[3]);
 				blk_acc = __vimax3_s16x2(blk_acc, cmv[4], cmv[5]);
 				blk_acc = __vimax3_s16x2(blk_acc, cmv[6], cmv[7]);
-				if (((sL + U) & (SSW_CM_BLOCK - 1)) == 0 || sL + U >= it.p1) {
-					colmax[it.cm_off + (sL / SSW_CM_BLOCK)] = blk_acc;
-					blk_acc = 0;
-				}
 			}
 		}
 		if (TERM) {

@@ -237,6 +237,11 @@ typedef struct {
 	int64_t leftover_pairs;      /* ssw_engine_search: pairs outside the device-planned grid (general path, selection on the host) */
 } ssw_engine_timing;
 int ssw_engine_last_timing(const ssw_engine* e, ssw_engine_timing* t);
+/* Column maxima of the engine's last forward fill launch, for tests: packed s16x2 words (the two alignments of a pair-task),
+ * pair-task after pair-task in launch order, (refLen + 3) / 4 * 4 words per pair-task (one per column), or in block mode
+ * (refLen / 64 + 4) / 4 * 4 (one per 64 columns; the words after the last block are not written).  Copies up to n_words
+ * into out and returns the number of words of that launch, -1 on error. */
+int64_t ssw_engine_last_colmax(ssw_engine* e, uint32_t* out, int64_t n_words);
 
 /*
  * Tuning knobs for tests and measurements; none of them changes a result.  Unknown names return -1.  Every engine has
