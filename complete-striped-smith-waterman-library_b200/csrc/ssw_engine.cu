@@ -31,6 +31,7 @@
 #include "ssw_grid.cuh"
 #include "ssw_text.cuh"
 #include "ssw_mark.cuh"
+#include "ssw_hits.h"
 #include "../../include/ssw_batch.h"
 
 #include <chrono>
@@ -1366,12 +1367,18 @@ static int emul_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Aln>&
 /* ------------------------------------------------------------------------------------------- */
 
 
+struct SearchHit { int32_t r; ssw_batch_result rec; };
+
 /* Top-k search on the grid path (ssw_engine_search): a selection kernel replaces the emit kernel, and an n_q x k hit table on the
- * device replaces the n_pairs records.  Filled by grid_scores: each query's hits among the pairs that are final on the grid. */
+ * device replaces the n_pairs records.  Filled by grid_scores: each query's hits among the pairs that are final on the grid.
+ * k == 0 is the threshold search (ssw_engine_search_all): a count and a compaction kernel replace the emit kernel, and every
+ * hit of a launch group is copied back, in reference order, while the next group computes. */
 struct GridSearch {
 	int32_t k, min_score;                   /* min_score >= 1 */
+	int64_t max_hits = 0;                   /* k == 0: more hits on the grid than this end the call (-2) */
 	std::vector<int32_t> hit_ref, n_hits;   /* n_q * k, n_q */
 	std::vector<ssw_batch_result> hits;     /* n_q * k */
+	std::vector<std::vector<SearchHit>> rows;   /* k == 0: n_q rows of grid hits in ascending reference index (the caller's) */
 	std::vector<uint8_t> q_on, r_on;        /* n_q, n_r: the grid path computed the pairs (q, r) with q_on[q] && r_on[r] */
 };
 
@@ -1443,7 +1450,11 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 	const size_t o_qp = o_perm + (4 * (size_t)n_r + 255) / 256 * 256;
 	const size_t o_cnt = o_qp + (8 * (size_t)(n_q / 2 + 1) + 255) / 256 * 256, o_list = o_cnt + 256;
 	const int32_t redo_cap = (int32_t)std::min<int64_t>((int64_t)n_qe * n_r, 1 << 22);
-	if (e->d_grid.ensure(o_list + 4 * (size_t)redo_cap)) return -1;
+	/* threshold search: behind the redo list, the hit counts of a launch group's query slots and their exclusive prefix */
+	const bool all = gs && gs->k == 0;
+	const size_t n_slots = all ? 2 * (size_t)(n_q / 2 + 1) : 0;
+	const size_t o_scnt = o_list + (4 * (size_t)redo_cap + 255) / 256 * 256, o_soff = o_scnt + (4 * n_slots + 255) / 256 * 256;
+	if (e->d_grid.ensure(all ? o_soff + 8 * (n_slots + 1) : o_list + 4 * (size_t)redo_cap)) return -1;
 	uint8_t* gb = e->d_grid.as<uint8_t>();
 	SSW_CUDA_OK(cudaMemcpyAsync(gb + o_qt, qt.data(), sizeof(SswGridQ) * n_q, cudaMemcpyHostToDevice, e->stream));
 	SSW_CUDA_OK(cudaMemcpyAsync(gb + o_roff, g_off.data(), 8 * (size_t)n_r, cudaMemcpyHostToDevice, e->stream));
@@ -1453,8 +1464,33 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 	SSW_CUDA_OK(cudaMemsetAsync(gb + o_cnt, 0, 256, e->stream));
 	/* search: [hits n_q*k][hit_ref n_q*k][n_hits n_q], every row written by the selection kernel of its query */
 	const size_t o_href = sizeof(ssw_batch_result) * (size_t)n_q * (gs ? gs->k : 0), o_nh = o_href + 4 * (size_t)n_q * (gs ? gs->k : 0);
-	if (gs ? e->d_hits.ensure(o_nh + 4 * (size_t)n_q) : e->d_out.ensure(sizeof(ssw_batch_result) * (size_t)n_pairs)) return -1;
-	if (gs) SSW_CUDA_OK(cudaMemsetAsync(e->d_hits.as<uint8_t>() + o_nh, 0, 4 * (size_t)n_q, e->stream));   /* queries off the grid: no hits here */
+	if (all) {
+		/* the hits of one launch group at a time, in e->d_hits (grown per group) */
+	} else if (gs ? e->d_hits.ensure(o_nh + 4 * (size_t)n_q) : e->d_out.ensure(sizeof(ssw_batch_result) * (size_t)n_pairs)) return -1;
+	if (gs && !all) SSW_CUDA_OK(cudaMemsetAsync(e->d_hits.as<uint8_t>() + o_nh, 0, 4 * (size_t)n_q, e->stream));   /* queries off the grid: no hits here */
+	/* threshold search: the group whose hits are still on the device, and a copy that brings them to gs->rows.  The device buffer
+	 * is written by the next group's compaction only after this copy has returned, so one buffer serves every group. */
+	struct HitGroup { int64_t n = 0; std::vector<int64_t> off; std::vector<int32_t> q; cudaEvent_t ev = nullptr; };
+	HitGroup pend;
+	int64_t grid_hits = 0;
+	if (all) gs->rows.assign((size_t)n_q, std::vector<SearchHit>());
+	auto flush_hits = [&]() -> int {
+		if (pend.n == 0) return 0;
+		if (!e->side[0]) SSW_CUDA_OK(cudaStreamCreateWithFlags(&e->side[0], cudaStreamNonBlocking));
+		SSW_CUDA_OK(cudaStreamWaitEvent(e->side[0], pend.ev, 0));
+		std::vector<ssw_batch_result> h((size_t)pend.n);
+		std::vector<int32_t> hr((size_t)pend.n);
+		const size_t o_ref = (sizeof(ssw_batch_result) * (size_t)pend.n + 255) / 256 * 256;
+		if (e->staged.copy(h.data(), e->d_hits.p, sizeof(ssw_batch_result) * (size_t)pend.n, e->side[0])) return -1;
+		if (e->staged.copy(hr.data(), e->d_hits.as<uint8_t>() + o_ref, 4 * (size_t)pend.n, e->side[0])) return -1;
+		for (size_t s = 0; s < pend.q.size(); ++s) {
+			if (pend.q[s] < 0) continue;
+			std::vector<SearchHit>& row = gs->rows[pend.q[s]];
+			for (int64_t i = pend.off[s]; i < pend.off[s + 1]; ++i) row.push_back(SearchHit{rsel[hr[i]], h[i]});   /* rsel ascending: order kept */
+		}
+		pend = HitGroup();
+		return 0;
+	};
 
 	const size_t free_b = ssw_free_device_bytes();
 	const size_t budget = std::max<size_t>((size_t)256 << 20, ssw_budget_share(free_b + e->d_colmax.cap + e->d_items.cap + e->d_alns.cap + e->d_res.cap));
@@ -1538,6 +1574,11 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 				           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
 				           (const SswFillResult*)e->d_res.as<SswFillResult>(), e->d_out.as<ssw_batch_result>(),
 				           reinterpret_cast<int32_t*>(gb + o_list), reinterpret_cast<int32_t*>(gb + o_cnt), redo_cap);
+			else if (all)
+				ssw_launch(ssw_grid_count_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream, A,
+				           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
+				           (const SswFillResult*)e->d_res.as<SswFillResult>(), gs->min_score, reinterpret_cast<int32_t*>(gb + o_scnt),
+				           reinterpret_cast<int32_t*>(gb + o_list), reinterpret_cast<int32_t*>(gb + o_cnt), redo_cap);
 			else {
 				uint8_t* hb = e->d_hits.as<uint8_t>();
 				ssw_launch(ssw_grid_select_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream, A,
@@ -1577,12 +1618,45 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 				continue;
 			}
 		}
+		if (all) {
+			/* the previous group's hits come back while this group computes; then this group's counts, the one synchronisation
+			 * per group, and its compaction at their prefix */
+			if (flush_hits()) return -1;
+			HitGroup hg;
+			std::vector<int32_t> sn((size_t)2 * A.n_qp);
+			SSW_CUDA_OK(cudaMemcpyAsync(sn.data(), gb + o_scnt, 4 * sn.size(), cudaMemcpyDeviceToHost, e->stream));
+			SSW_CUDA_OK(cudaStreamSynchronize(e->stream));
+			hg.off.assign(sn.size() + 1, 0); hg.q.resize(sn.size());
+			for (size_t s = 0; s < sn.size(); ++s) { hg.q[s] = s & 1 ? qps[s / 2].y : qps[s / 2].x; hg.off[s + 1] = hg.off[s] + sn[s]; }
+			hg.n = hg.off.back();
+			grid_hits += hg.n;
+			if (grid_hits > gs->max_hits) return -2;
+			if (hg.n > 0) {
+				const size_t o_ref = (sizeof(ssw_batch_result) * (size_t)hg.n + 255) / 256 * 256;
+				if (e->d_hits.ensure(o_ref + 4 * (size_t)hg.n)) return -1;
+				uint8_t* hb = e->d_hits.as<uint8_t>();
+				SSW_CUDA_OK(cudaMemcpyAsync(gb + o_soff, hg.off.data(), 8 * hg.off.size(), cudaMemcpyHostToDevice, e->stream));
+				e->laps.start(e->stream);
+				ssw_launch(ssw_grid_compact_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream, A,
+				           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
+				           (const SswFillResult*)e->d_res.as<SswFillResult>(), gs->min_score, (const int64_t*)reinterpret_cast<int64_t*>(gb + o_soff),
+				           reinterpret_cast<int32_t*>(hb + o_ref), reinterpret_cast<ssw_batch_result*>(hb));
+				SSW_CUDA_OK(cudaGetLastError());
+				e->laps.stop(e->stream, &e->timing.resolve_ms);
+				e->timing.other_launches += 1;
+				hg.ev = groups.back().ev;
+				SSW_CUDA_OK(cudaEventRecord(hg.ev, e->stream));
+			}
+			pend = std::move(hg);
+		}
 		tr.lap("grid: launch group");
 	}
 	/* every launch is queued; bring the records back group by group on the copy stream while later groups still compute */
 	bool all_contiguous = !groups.empty();
 	for (const GridGroup& gg : groups) if (!gg.contiguous) all_contiguous = false;
-	if (gs) {
+	if (all) {
+		if (flush_hits()) return -1;                 /* the last group's hits */
+	} else if (gs) {
 		/* the hit table in one copy (rows of a rejected pilot group were overwritten by their second run) */
 		std::vector<uint8_t> h(o_nh + 4 * (size_t)n_q);
 		if (e->staged.copy(h.data(), e->d_hits.p, h.size(), e->stream)) return -1;
@@ -1592,6 +1666,8 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 		memcpy(gs->n_hits.data(), h.data() + o_nh, 4 * (size_t)n_q);
 		for (int32_t q : order)
 			for (int32_t i = 0; i < gs->n_hits[q]; ++i) { int32_t& r = gs->hit_ref[(size_t)q * gs->k + i]; r = rsel[r]; }
+	}
+	if (gs) {
 		gs->q_on.assign((size_t)n_q, 0); gs->r_on.assign((size_t)n_r_all, 0);
 		for (int32_t q : order) gs->q_on[q] = 1;
 		for (int32_t r : rsel) gs->r_on[r] = 1;
@@ -1951,8 +2027,6 @@ extern "C" int ssw_engine_align(ssw_engine* e, const ssw_batch_params* params,
 /* top-k search over the full grid                                                               */
 /* ------------------------------------------------------------------------------------------- */
 
-struct SearchHit { int32_t r; ssw_batch_result rec; };
-
 /* the rank order of ssw_engine_search: status-1 pairs first (their score is at least the byte limit), then score1 descending,
  * then reference ascending -- a total order, so the k best do not depend on how the grid was cut */
 static bool hit_before(const SearchHit& a, const SearchHit& b)
@@ -1973,19 +2047,27 @@ static void keep_best(std::vector<SearchHit>& v, int32_t k)
 /* general path of a search: pairs per block of whole queries */
 #define SSW_SEARCH_BLOCK_PAIRS ((int64_t)1 << 22)
 
-static int engine_search_impl(ssw_engine* e, const ssw_batch_params* params, int32_t k, int32_t min_score,
-                              int32_t* hit_ref, ssw_batch_result* hits, int32_t* n_hits,
-                              uint32_t* cigar_pool, int64_t pool_cap, int64_t* pool_used)
+/* worst-case CIGAR words of one pair (the bound of the device groups): a path has at most query span + reference span + 2
+ * words, and a positive-scoring path cannot delete more than query length * max score / gap_extend bases */
+static int64_t cigar_words_bound(int64_t ql, int64_t rl, int gap_extend)
 {
-	if (!e || !params || !params->mat) { fprintf(stderr, "[libssw-b200] ssw_engine_search: no engine or no parameters\n"); return -1; }
-	if (k < 1 || k > SSW_SEARCH_MAX_K) { fprintf(stderr, "[libssw-b200] ssw_engine_search: k = %d outside 1 .. %d\n", k, SSW_SEARCH_MAX_K); return -1; }
-	if (!hit_ref || !hits || !n_hits) { fprintf(stderr, "[libssw-b200] ssw_engine_search: NULL output array\n"); return -1; }
-	if (e->n_q <= 0 || e->n_r <= 0) { fprintf(stderr, "[libssw-b200] ssw_engine_search: no resident sequences\n"); return -1; }
-	const ssw_batch_params& P = *params;
-	if (P.n < 1 || P.n > 64) { fprintf(stderr, "[libssw-b200] alphabet size %d not supported (1..64)\n", P.n); return -1; }
-	int64_t pool_used_local = 0, no_pool = 0;
-	if (!pool_used) pool_used = &pool_used_local;
-	*pool_used = 0;
+	int64_t span = rl;
+	if (gap_extend > 0) { const int64_t b = ql + ql * 127 / gap_extend; if (b < span) span = b; }
+	return ql + span + 4;
+}
+
+static bool ref_before(const SearchHit& a, const SearchHit& b) { return a.r < b.r; }
+
+/* The rows of a search over the full grid, shared by the top-k search (keep = k: a row holds its k best hits in rank order)
+ * and the threshold search (keep = 0: every hit, in ascending reference index).  The grid path takes what it can; the pairs
+ * it re-does and the pairs it leaves over run through the general path and are merged into their rows (disjoint sets, so a
+ * merge of sorted lists); with a flag, the caller's params run once more on the kept pairs only, their CIGARs going to
+ * cigar_pool or, with own_pool, to a pool sized for them.  keep = 0 and more than max_hits hits: -2. */
+static int search_rows(ssw_engine* e, const ssw_batch_params& P, int32_t keep, int32_t min_score, int64_t max_hits,
+                       std::vector<std::vector<SearchHit>>& best, uint32_t* cigar_pool, int64_t pool_cap, int64_t* pool_used,
+                       std::vector<uint32_t>* own_pool)
+{
+	int64_t no_pool = 0;
 	SSW_CUDA_OK(cudaSetDevice(e->device));
 	memset(&e->timing, 0, sizeof(e->timing));
 	e->laps.laps.clear(); e->laps.used = 0;
@@ -1996,27 +2078,40 @@ static int engine_search_impl(ssw_engine* e, const ssw_batch_params* params, int
 	/* the ranking runs on flag-0 records: score1, the ends and the second best do not depend on the flag */
 	ssw_batch_params P0 = P;
 	P0.flag = 0;
-	std::vector<std::vector<SearchHit>> best((size_t)n_q);
+	best.assign((size_t)n_q, std::vector<SearchHit>());
+	int64_t n_kept = 0;                              /* keep = 0: the hits so far */
+	/* a row after a merge: its k best in rank order, or -- a sorted row followed by sorted additions -- one merge by reference */
+	auto settle = [&](int32_t q) {
+		std::vector<SearchHit>& v = best[q];
+		if (keep > 0) keep_best(v, keep);
+		else std::inplace_merge(v.begin(), std::is_sorted_until(v.begin(), v.end(), ref_before), v.end(), ref_before);
+	};
 	GridSearch gs;
-	gs.k = k; gs.min_score = thr;
+	gs.k = keep; gs.min_score = thr; gs.max_hits = max_hits;
 	std::vector<int32_t> redo;
 	int rc = grid_scores(e, P0, S, (int64_t)n_q * n_r, nullptr, &redo, &gs);
 	if (rc < 0) return rc;
 	if (rc == 1) {
-		for (int32_t q = 0; q < n_q; ++q)
-			for (int32_t i = 0; i < gs.n_hits[q]; ++i) best[q].push_back(SearchHit{gs.hit_ref[(size_t)q * k + i], gs.hits[(size_t)q * k + i]});
+		if (keep > 0) {
+			for (int32_t q = 0; q < n_q; ++q)
+				for (int32_t i = 0; i < gs.n_hits[q]; ++i) best[q].push_back(SearchHit{gs.hit_ref[(size_t)q * keep + i], gs.hits[(size_t)q * keep + i]});
+		} else {
+			best.swap(gs.rows);
+			for (const std::vector<SearchHit>& v : best) n_kept += (int64_t)v.size();
+		}
 		/* pairs the grid left to the general path, merged per query: the k best of all pairs are the k best of the grid's k best
 		 * and the re-done pairs, whatever the reason of the re-do */
 		if (!redo.empty()) {
 			std::vector<int32_t> pq(redo.size()), pr(redo.size());
 			for (size_t i = 0; i < redo.size(); ++i) { pq[i] = redo[i] / n_r; pr[i] = redo[i] % n_r; }
 			std::vector<ssw_batch_result> sub(redo.size());
-			const ssw_engine_timing keep = e->timing;
+			const ssw_engine_timing keep_t = e->timing;
 			rc = align_general(e, P0, S, (int64_t)redo.size(), pq.data(), pr.data(), sub.data(), nullptr, 0, &no_pool);
 			if (rc) return rc;
-			e->timing.byte_overflows = keep.byte_overflows + (int64_t)redo.size();
-			for (size_t i = 0; i < redo.size(); ++i) if (is_hit(sub[i], thr)) best[pq[i]].push_back(SearchHit{pr[i], sub[i]});
-			for (int32_t q = 0; q < n_q; ++q) keep_best(best[q], k);
+			e->timing.byte_overflows = keep_t.byte_overflows + (int64_t)redo.size();
+			for (size_t i = 0; i < redo.size(); ++i) if (is_hit(sub[i], thr)) { best[pq[i]].push_back(SearchHit{pr[i], sub[i]}); ++n_kept; }
+			if (keep == 0 && n_kept > max_hits) return -2;
+			for (int32_t q = 0; q < n_q; ++q) settle(q);
 		}
 	} else {
 		gs.q_on.assign((size_t)n_q, 0); gs.r_on.assign((size_t)n_r, 0);       /* no grid: every pair is left over */
@@ -2046,16 +2141,25 @@ static int engine_search_impl(ssw_engine* e, const ssw_batch_params* params, int
 			if (rc) return rc;
 			e->timing.byte_overflows += over;
 			e->timing.leftover_pairs += m;
-			for (int64_t i = 0; i < m; ++i) if (is_hit(rec[i], thr)) best[pq[i]].push_back(SearchHit{pr[i], rec[i]});
-			for (int32_t q = q0; q < q1; ++q) keep_best(best[q], k);
+			for (int64_t i = 0; i < m; ++i) if (is_hit(rec[i], thr)) { best[pq[i]].push_back(SearchHit{pr[i], rec[i]}); ++n_kept; }
+			if (keep == 0 && n_kept > max_hits) return -2;
+			for (int32_t q = q0; q < q1; ++q) settle(q);
 		}
 		q0 = q1;
 	}
-	/* the caller's flag: begins and CIGARs of the hits only (at most n_q * k pairs) */
+	/* the caller's flag: begins and CIGARs of the kept hits only */
 	if (P.flag != 0) {
 		std::vector<int32_t> hq, hr;
 		for (int32_t q = 0; q < n_q; ++q) for (const SearchHit& h : best[q]) { hq.push_back(q); hr.push_back(h.r); }
 		if (!hq.empty()) {
+			std::unique_ptr<uint32_t[]> own;
+			if (own_pool && (P.flag & 7)) {
+				pool_cap = 8;
+				for (size_t i = 0; i < hq.size(); ++i)
+					pool_cap += cigar_words_bound(e->q_off[hq[i] + 1] - e->q_off[hq[i]], e->r_len[hr[i]], P.gap_extend);
+				own.reset(new uint32_t[(size_t)pool_cap]);      /* worst-case sized and mostly untouched: uninitialised storage */
+				cigar_pool = own.get();
+			}
 			std::vector<ssw_batch_result> rec(hq.size());
 			const int64_t over = e->timing.byte_overflows;
 			rc = align_general(e, P, S, (int64_t)hq.size(), hq.data(), hr.data(), rec.data(), cigar_pool, pool_cap, pool_used);
@@ -2063,12 +2167,34 @@ static int engine_search_impl(ssw_engine* e, const ssw_batch_params* params, int
 			e->timing.byte_overflows = over;
 			size_t j = 0;
 			for (int32_t q = 0; q < n_q; ++q) for (SearchHit& h : best[q]) h.rec = rec[j++];
+			if (own) own_pool->assign(own.get(), own.get() + *pool_used);
 		}
 	}
+	e->timing.total_ms = e->t_total.stop(e->stream);
+	e->laps.collect();
+	return 0;
+}
+
+static int engine_search_impl(ssw_engine* e, const ssw_batch_params* params, int32_t k, int32_t min_score,
+                              int32_t* hit_ref, ssw_batch_result* hits, int32_t* n_hits,
+                              uint32_t* cigar_pool, int64_t pool_cap, int64_t* pool_used)
+{
+	if (!e || !params || !params->mat) { fprintf(stderr, "[libssw-b200] ssw_engine_search: no engine or no parameters\n"); return -1; }
+	if (k < 1 || k > SSW_SEARCH_MAX_K) { fprintf(stderr, "[libssw-b200] ssw_engine_search: k = %d outside 1 .. %d\n", k, SSW_SEARCH_MAX_K); return -1; }
+	if (!hit_ref || !hits || !n_hits) { fprintf(stderr, "[libssw-b200] ssw_engine_search: NULL output array\n"); return -1; }
+	if (e->n_q <= 0 || e->n_r <= 0) { fprintf(stderr, "[libssw-b200] ssw_engine_search: no resident sequences\n"); return -1; }
+	const ssw_batch_params& P = *params;
+	if (P.n < 1 || P.n > 64) { fprintf(stderr, "[libssw-b200] alphabet size %d not supported (1..64)\n", P.n); return -1; }
+	int64_t pool_used_local = 0;
+	if (!pool_used) pool_used = &pool_used_local;
+	*pool_used = 0;
+	std::vector<std::vector<SearchHit>> best;
+	const int rc = search_rows(e, P, k, min_score, 0, best, cigar_pool, pool_cap, pool_used, nullptr);
+	if (rc) return rc;
 	ssw_batch_result none;
 	memset(&none, 0, sizeof(none));
 	none.ref_begin1 = -1; none.read_begin1 = -1; none.cigar_off = -1;
-	for (int32_t q = 0; q < n_q; ++q) {
+	for (int32_t q = 0; q < e->n_q; ++q) {
 		const std::vector<SearchHit>& v = best[q];
 		n_hits[q] = (int32_t)v.size();
 		for (int32_t i = 0; i < k; ++i) {
@@ -2077,8 +2203,6 @@ static int engine_search_impl(ssw_engine* e, const ssw_batch_params* params, int
 			hits[(size_t)q * k + i] = used ? v[i].rec : none;
 		}
 	}
-	e->timing.total_ms = e->t_total.stop(e->stream);
-	e->laps.collect();
 	return 0;
 }
 
@@ -2090,6 +2214,62 @@ extern "C" int ssw_engine_search(ssw_engine* e, const ssw_batch_params* params, 
 	catch (const std::exception& ex) { fprintf(stderr, "[libssw-b200] ssw_engine_search: %s\n", ex.what()); return -1; }
 	catch (...) { return -1; }
 }
+
+/* ------------------------------------------------------------------------------------------- */
+/* threshold search over the full grid: every hit, as a CSR matrix in pair order                  */
+/* ------------------------------------------------------------------------------------------- */
+
+static int engine_search_all_impl(ssw_engine* e, const ssw_batch_params* params, int32_t min_score, int64_t max_hits, ssw_hit_set** out)
+{
+	if (!out) { fprintf(stderr, "[libssw-b200] ssw_engine_search_all: NULL output\n"); return -1; }
+	*out = nullptr;
+	if (!e || !params || !params->mat) { fprintf(stderr, "[libssw-b200] ssw_engine_search_all: no engine or no parameters\n"); return -1; }
+	if (max_hits < 0) { fprintf(stderr, "[libssw-b200] ssw_engine_search_all: max_hits = %lld is negative\n", (long long)max_hits); return -1; }
+	if (e->n_q <= 0 || e->n_r <= 0) { fprintf(stderr, "[libssw-b200] ssw_engine_search_all: no resident sequences\n"); return -1; }
+	const ssw_batch_params& P = *params;
+	if (P.n < 1 || P.n > 64) { fprintf(stderr, "[libssw-b200] alphabet size %d not supported (1..64)\n", P.n); return -1; }
+	std::unique_ptr<ssw_hit_set> s(new ssw_hit_set());
+	std::vector<std::vector<SearchHit>> best;
+	int64_t used = 0;
+	const int rc = search_rows(e, P, 0, min_score, max_hits, best, nullptr, 0, &used, &s->pool);
+	if (rc == -2) fprintf(stderr, "[libssw-b200] ssw_engine_search_all: more than max_hits = %lld hits\n", (long long)max_hits);
+	if (rc) return rc;
+	s->n_rows = e->n_q;
+	s->row_off.assign((size_t)e->n_q + 1, 0);
+	for (int32_t q = 0; q < e->n_q; ++q) s->row_off[q + 1] = s->row_off[q] + (int64_t)best[q].size();
+	const size_t n = (size_t)s->row_off.back();
+	s->hit_ref.resize(n); s->hits.resize(n);
+	size_t j = 0;
+	for (std::vector<SearchHit>& v : best) {
+		for (const SearchHit& h : v) { s->hit_ref[j] = h.r; s->hits[j] = h.rec; ++j; }
+		std::vector<SearchHit>().swap(v);
+	}
+	*out = s.release();
+	return 0;
+}
+
+extern "C" int ssw_engine_search_all(ssw_engine* e, const ssw_batch_params* params, int32_t min_score, int64_t max_hits, ssw_hit_set** out)
+{
+	if (out) *out = nullptr;
+	try { SswBusyGuard busy(e ? e->device : 0); return engine_search_all_impl(e, params, min_score, max_hits, out); }
+	catch (const std::exception& ex) { fprintf(stderr, "[libssw-b200] ssw_engine_search_all: %s\n", ex.what()); return -1; }
+	catch (...) { return -1; }
+}
+
+extern "C" int ssw_hit_set_view(const ssw_hit_set* s, ssw_hit_view* v)
+{
+	if (!s || !v) { fprintf(stderr, "[libssw-b200] ssw_hit_set_view: NULL argument\n"); return -1; }
+	v->n_rows = s->n_rows;
+	v->n_hits = (int64_t)s->hits.size();
+	v->row_off = s->row_off.data();
+	v->hit_ref = s->hit_ref.empty() ? nullptr : s->hit_ref.data();
+	v->hits = s->hits.empty() ? nullptr : s->hits.data();
+	v->cigar_pool = s->pool.empty() ? nullptr : s->pool.data();
+	v->pool_used = (int64_t)s->pool.size();
+	return 0;
+}
+
+extern "C" void ssw_hit_set_destroy(ssw_hit_set* s) { delete s; }
 
 /* mark_mismatch (ssw.c:1019-1074) for the CIGARs of a batch, on the device (ssw_mark.cuh) */
 static int mark_mismatch_impl(ssw_engine* e, int64_t n_pairs, const int32_t* pair_query, const int32_t* pair_ref,

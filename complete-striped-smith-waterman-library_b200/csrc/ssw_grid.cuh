@@ -9,7 +9,7 @@
  * index, and maps the indices back on the host), and the resolve output is written straight into the caller-visible
  * ssw_batch_result records.  Pairs whose byte-semantics score overflowed are appended to a list and re-done by the
  * general path.  A top-k search (ssw_engine_search) replaces the emit kernel by a selection kernel that keeps only each
- * query's k best records.
+ * query's k best records; a threshold search (ssw_engine_search_all) by a count and a compaction kernel that keep every hit.
  */
 #ifndef SSW_GRID_CUH
 #define SSW_GRID_CUH
@@ -260,6 +260,75 @@ ssw_grid_select_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGrid
 		hit_ref[(int64_t)q * k + i] = r;
 	}
 	if (tid == 0) n_hits[q] = cnt;
+}
+
+/* ---- threshold search (ssw_engine_search_all): every hit, compacted in reference order ----------------------------------- */
+
+/* One CTA per query slot (pi, half) of a launch group, as the selection kernel: slot_n[slot] receives the number of hits of
+ * that query among the group's resolve results (0 for a slot without a query).  The only kernel of the threshold search that
+ * queues redo pairs: each pair of the group is visited once, so each is queued once. */
+__global__ void __launch_bounds__(SSW_SELECT_THREADS)
+ssw_grid_count_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGridQ* __restrict__ qt,
+                      const SswFillResult* __restrict__ res, int32_t min_score, int32_t* __restrict__ slot_n,
+                      int32_t* __restrict__ redo_list, int32_t* __restrict__ redo_count, int32_t redo_cap)
+{
+	__shared__ int32_t s_n;
+	const int h = (int)(blockIdx.x & 1), pi = (int)(blockIdx.x >> 1);
+	const int2 pr = qp[pi];
+	const int q = h ? pr.y : pr.x;
+	const int tid = threadIdx.x;
+	if (q < 0) {                                       /* the whole CTA: no second query in this pair-task */
+		if (tid == 0) slot_n[blockIdx.x] = 0;
+		return;
+	}
+	const int mask_len = qt[q].mask_len;
+	const int n_r = A.n_r;
+	const SswFillResult* rq = res + (int64_t)pi * n_r * 2 + h;
+	const int64_t p0 = (int64_t)q * n_r;
+	if (tid == 0) s_n = 0;
+	__syncthreads();
+	int c = 0;
+	for (int r = tid; r < n_r; r += SSW_SELECT_THREADS) {
+		ssw_batch_result o;
+		if (ssw_grid_record<true>(rq[2 * (int64_t)r], mask_len, p0 + r, o, redo_list, redo_count, redo_cap) && o.score1 >= min_score) ++c;
+	}
+	if (c) atomicAdd(&s_n, c);
+	__syncthreads();
+	if (tid == 0) slot_n[blockIdx.x] = s_n;
+}
+
+/* Same layout: the hits of a slot in reference order, written contiguously from slot_off[slot] (the host's exclusive prefix of
+ * the counts over the group's slots): one ordered ballot pass, as pass 3 of the selection kernel, which stops once the slot's
+ * count is reached.  Records and device reference numbers. */
+__global__ void __launch_bounds__(SSW_SELECT_THREADS)
+ssw_grid_compact_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGridQ* __restrict__ qt,
+                        const SswFillResult* __restrict__ res, int32_t min_score, const int64_t* __restrict__ slot_off,
+                        int32_t* __restrict__ hit_ref, ssw_batch_result* __restrict__ hits)
+{
+	__shared__ int32_t s_warp[2][SSW_SELECT_THREADS / 32];
+	const int h = (int)(blockIdx.x & 1), pi = (int)(blockIdx.x >> 1);
+	const int2 pr = qp[pi];
+	const int q = h ? pr.y : pr.x;
+	if (q < 0) return;
+	const int mask_len = qt[q].mask_len;
+	const int n_r = A.n_r, tid = threadIdx.x;
+	const SswFillResult* rq = res + (int64_t)pi * n_r * 2 + h;
+	const int64_t p0 = (int64_t)q * n_r;
+	const int64_t base = slot_off[blockIdx.x], cnt = slot_off[blockIdx.x + 1] - base;
+	int64_t done = 0;
+	/* two prefix buffers in turn: a step's writes to one cannot race the reads of the step before, which a barrier separates */
+	for (int r0 = 0, it = 0; r0 < n_r && done < cnt; r0 += SSW_SELECT_THREADS, ++it) {
+		const int r = r0 + tid;
+		ssw_batch_result o;
+		const bool hit = r < n_r && ssw_grid_record<false>(rq[2 * (int64_t)r], mask_len, p0 + r, o, nullptr, nullptr, 0) && o.score1 >= min_score;
+		int n = 0;
+		const int at = ssw_block_prefix(hit, s_warp[it & 1], &n);
+		if (hit) {
+			hits[base + done + at] = o;
+			hit_ref[base + done + at] = r;
+		}
+		done += n;
+	}
 }
 
 #endif /* SSW_GRID_CUH */

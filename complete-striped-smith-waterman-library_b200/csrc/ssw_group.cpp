@@ -18,6 +18,7 @@
 
 #include "../../include/ssw.h"
 #include "../../include/ssw_batch.h"
+#include "ssw_hits.h"
 
 s_align* ssw_record_from(const ssw_batch_result& r, const uint32_t* pool);       /* ssw_capi.cu */
 
@@ -384,6 +385,104 @@ extern "C" int ssw_group_search(ssw_group* g, const ssw_batch_params* params, co
 		return 0;
 	}
 	catch (const std::exception& ex) { fprintf(stderr, "[libssw-b200] ssw_group_search: %s\n", ex.what()); return -1; }
+	catch (...) { return -1; }
+}
+
+extern "C" int ssw_group_search_all(ssw_group* g, const ssw_batch_params* params, const int8_t* table, int32_t add_reverse_complement,
+                                    int32_t n_queries, const void* queries, const int64_t* query_off,
+                                    int32_t n_refs, const void* refs, const int64_t* ref_off,
+                                    int32_t min_score, int64_t max_hits, ssw_hit_set** out)
+{
+	if (!out) { fprintf(stderr, "[libssw-b200] ssw_group_search_all: NULL output\n"); return -1; }
+	*out = nullptr;
+	if (!g || g->eng.empty() || !params || !params->mat) { fprintf(stderr, "[libssw-b200] ssw_group_search_all: NULL argument\n"); return -1; }
+	if (max_hits < 0) { fprintf(stderr, "[libssw-b200] ssw_group_search_all: max_hits = %lld is negative\n", (long long)max_hits); return -1; }
+	if (n_queries <= 0 || n_refs <= 0 || !queries || !refs || !query_off || !ref_off) { fprintf(stderr, "[libssw-b200] ssw_group_search_all: no sequences\n"); return -1; }
+	struct Part {
+		int32_t q0 = 0, nq = 0;      /* first query and queries of the block; its set has nq (or 2 nq) rows */
+		ssw_hit_set* set = nullptr;
+		int rc = 0;
+		Part() = default;
+		Part(const Part&) = delete;
+		Part& operator=(const Part&) = delete;
+		~Part() { ssw_hit_set_destroy(set); }
+	};
+	try {
+		const ssw_batch_params& P = *params;
+		for (int32_t q = 0; q < n_queries; ++q) if (query_off[q + 1] < query_off[q]) { fprintf(stderr, "[libssw-b200] query offsets are not non-decreasing at %d\n", q); return -1; }
+		for (int32_t r = 0; r < n_refs; ++r) if (ref_off[r + 1] < ref_off[r]) { fprintf(stderr, "[libssw-b200] reference offsets are not non-decreasing at %d\n", r); return -1; }
+		const bool add_rc = table && add_reverse_complement;
+		/* the queries cut as for ssw_group_search; every device searches its block against all references */
+		const int world = (int)g->eng.size();
+		const std::vector<int64_t> b = balanced_bounds(n_queries, world, [&](int64_t q) { return query_off[q + 1] - query_off[q] + 1; });
+		std::vector<Part> parts((size_t)world);
+		auto work = [&](int d) {
+			Part& S = parts[d];
+			try {
+				S.q0 = (int32_t)b[d];
+				S.nq = (int32_t)(b[d + 1] - b[d]);
+				if (S.nq <= 0) return;
+				std::vector<int64_t> qoff((size_t)S.nq + 1);
+				for (int32_t j = 0; j <= S.nq; ++j) qoff[j] = query_off[S.q0 + j] - query_off[S.q0];
+				const char* qbase = (const char*)queries + query_off[S.q0];
+				ssw_engine* e = g->eng[d];
+				S.rc = table ? ssw_engine_set_sequences_text(e, S.nq, qbase, qoff.data(), n_refs, (const char*)refs, ref_off, table, P.n, add_rc ? 1 : 0)
+				             : ssw_engine_set_sequences(e, S.nq, (const int8_t*)qbase, qoff.data(), n_refs, (const int8_t*)refs, ref_off);
+				if (S.rc) return;
+				S.rc = ssw_engine_search_all(e, &P, min_score, max_hits, &S.set);      /* each block alone is bounded by the total's bound */
+			}
+			catch (const std::exception& ex) { fprintf(stderr, "[libssw-b200] device group: %s\n", ex.what()); S.rc = -1; }
+			catch (...) { S.rc = -1; }
+		};
+#ifdef SSW_CPU_EMU
+		for (int d = 0; d < world; ++d) work(d);        /* the emulator's fibers are not thread-safe */
+#else
+		{
+			std::vector<std::thread> th;
+			th.reserve((size_t)world);
+			for (int d = 1; d < world; ++d) {
+				try { th.emplace_back(work, d); }
+				catch (...) { work(d); }                 /* no thread to be had: this block runs here */
+			}
+			work(0);
+			for (std::thread& t : th) t.join();
+		}
+#endif
+		for (const Part& S : parts) if (S.rc) return S.rc;
+		int64_t n_hits = 0, n_words = 0;
+		for (const Part& S : parts) if (S.set) { n_hits += (int64_t)S.set->hits.size(); n_words += (int64_t)S.set->pool.size(); }
+		if (n_hits > max_hits) { fprintf(stderr, "[libssw-b200] ssw_group_search_all: more than max_hits = %lld hits\n", (long long)max_hits); return -2; }
+		if (n_words > 0x7fffffff) { fprintf(stderr, "[libssw-b200] more than 2^31 CIGAR words in one batch: split the batch\n"); return -1; }
+		/* rows in query order -- every block's queries, then (reverse complements) every block's second half -- keep pair order */
+		std::unique_ptr<ssw_hit_set> s(new ssw_hit_set());
+		s->n_rows = n_queries * (add_rc ? 2 : 1);
+		s->row_off.reserve((size_t)s->n_rows + 1);
+		s->row_off.push_back(0);
+		s->hit_ref.reserve((size_t)n_hits); s->hits.reserve((size_t)n_hits); s->pool.reserve((size_t)n_words);
+		std::vector<int64_t> base((size_t)world, 0);
+		for (int d = 0; d < world; ++d) {
+			if (!parts[d].set) continue;
+			base[d] = (int64_t)s->pool.size();
+			s->pool.insert(s->pool.end(), parts[d].set->pool.begin(), parts[d].set->pool.end());
+		}
+		for (int half = 0; half < (add_rc ? 2 : 1); ++half)
+			for (int d = 0; d < world; ++d) {
+				const Part& S = parts[d];
+				if (!S.set) continue;
+				for (int32_t l = half * S.nq; l < (half + 1) * S.nq; ++l) {
+					for (int64_t i = S.set->row_off[l]; i < S.set->row_off[l + 1]; ++i) {
+						ssw_batch_result o = S.set->hits[i];
+						if (o.cigar_off >= 0) o.cigar_off += (int32_t)base[d];
+						s->hits.push_back(o);
+						s->hit_ref.push_back(S.set->hit_ref[i]);
+					}
+					s->row_off.push_back((int64_t)s->hits.size());
+				}
+			}
+		*out = s.release();
+		return 0;
+	}
+	catch (const std::exception& ex) { fprintf(stderr, "[libssw-b200] ssw_group_search_all: %s\n", ex.what()); return -1; }
 	catch (...) { return -1; }
 }
 

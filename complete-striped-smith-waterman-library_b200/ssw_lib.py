@@ -58,6 +58,45 @@ RESULT_DTYPE = np.dtype([("score1", "<u2"), ("score2", "<u2"), ("ref_begin1", "<
 assert RESULT_DTYPE.itemsize == 36
 
 
+class HitView(ct.Structure):
+    """ssw_hit_view (include/ssw_batch.h)."""
+    _fields_ = [("n_rows", ct.c_int32), ("n_hits", ct.c_int64), ("row_off", ct.c_void_p), ("hit_ref", ct.c_void_p),
+                ("hits", ct.c_void_p), ("cigar_pool", ct.c_void_p), ("pool_used", ct.c_int64)]
+
+
+# default bound of search_all: 2^26 hits, 2.7 GB of records and reference indices
+SEARCH_ALL_MAX_HITS = 1 << 26
+
+
+def _copy_out(ptr, n, dtype):
+    """n items of dtype at a C pointer, as an owned numpy array (copied as bytes: a copy of the structured record dtype goes
+    field by field, several times slower)"""
+    dtype = np.dtype(dtype)
+    if n <= 0 or not ptr:
+        return np.zeros(0, dtype=dtype)
+    return np.frombuffer((ct.c_char * (n * dtype.itemsize)).from_address(ptr), dtype=np.uint8).copy().view(dtype)
+
+
+def _take_hit_set(lib, rv, handle, name, max_hits):
+    """(row_off int64, hit_ref int32, hits RESULT_DTYPE, cigar_pool uint32) copied out of an ssw_hit_set, which is destroyed"""
+    if rv == -2:
+        raise RuntimeError("%s: more than max_hits = %d hits (raise max_hits or min_score)" % (name, max_hits))
+    if rv or not handle.value:
+        raise RuntimeError("%s failed (%d)" % (name, rv))
+    lib.ssw_hit_set_view.argtypes = [ct.c_void_p, ct.POINTER(HitView)]
+    lib.ssw_hit_set_view.restype = ct.c_int
+    lib.ssw_hit_set_destroy.argtypes = [ct.c_void_p]
+    lib.ssw_hit_set_destroy.restype = None
+    try:
+        v = HitView()
+        if lib.ssw_hit_set_view(handle, ct.byref(v)):
+            raise RuntimeError("ssw_hit_set_view failed")
+        return (_copy_out(v.row_off, v.n_rows + 1, np.int64), _copy_out(v.hit_ref, v.n_hits, np.int32),
+                _copy_out(v.hits, v.n_hits, RESULT_DTYPE), _copy_out(v.cigar_pool, v.pool_used, np.uint32))
+    finally:
+        lib.ssw_hit_set_destroy(handle)
+
+
 def _load(lib_dir=None, lib_name=LIB_NAME):
     path = op.join(lib_dir or _HERE, lib_name)
     if not op.exists(path):
@@ -272,6 +311,21 @@ class BatchAligner(object):
             raise RuntimeError("ssw_engine_search failed (%d)" % rv)
         return hit_ref, hits, n_hits, pool[: used.value]
 
+    def search_all(self, mat, n, min_score, max_hits=SEARCH_ALL_MAX_HITS, gap_open=3, gap_extend=1, flag=0, filters=0, filterd=0,
+                   mask_len=-1, score_size=2):
+        """Threshold search of every resident query against all resident references (ssw_engine_search_all): every hit
+        (status 1 or score1 >= max(min_score, 1)).  Returns (row_off[n_q + 1] int64, hit_ref int32, hits RESULT_DTYPE,
+        cigar_pool uint32) in CSR form: row q is [row_off[q], row_off[q + 1]), in ascending reference index.  More hits
+        than max_hits raise RuntimeError."""
+        f = self.lib.ssw_engine_search_all
+        f.argtypes = [ct.c_void_p, ct.POINTER(BatchParams), ct.c_int32, ct.c_int64, ct.POINTER(ct.c_void_p)]
+        f.restype = ct.c_int
+        mat, matp = _i8(mat)
+        P = BatchParams(matp, n, gap_open, gap_extend, flag, filters, filterd, mask_len, score_size)
+        handle = ct.c_void_p()
+        rv = f(self.h, ct.byref(P), int(min_score), int(max_hits), ct.byref(handle))
+        return _take_hit_set(self.lib, rv, handle, "ssw_engine_search_all", max_hits)
+
     def mark_mismatch(self, res, pool, pair_query=None, pair_ref=None):
         """mark_mismatch (ssw.c:1019-1074) for every CIGAR of a batch, on the device (ssw_engine_mark_mismatch): `res` / `pool`
         as returned by align() for the same pairs.  Returns (records with cigar_off / cigar_len pointing into the new pool,
@@ -467,3 +521,35 @@ class GroupAligner(object):
         if rv:
             raise RuntimeError("ssw_group_search failed (%d)" % rv)
         return hit_ref, hits, n_hits, pool[: used.value]
+
+    def search_all(self, queries, refs, mat, n, min_score, max_hits=SEARCH_ALL_MAX_HITS, gap_open=3, gap_extend=1, flag=0,
+                   filters=0, filterd=0, mask_len=-1, score_size=2, table=None, add_reverse_complement=False):
+        """BatchAligner.search_all over the devices of the group (ssw_group_search_all): sequences as for align().  Returns
+        (row_off, hit_ref, hits, cigar_pool); with add_reverse_complement the rows of the reverse complements follow those of
+        the queries."""
+        f = self.lib.ssw_group_search_all
+        f.argtypes = [ct.c_void_p, ct.POINTER(BatchParams), ct.POINTER(ct.c_int8), ct.c_int32,
+                      ct.c_int32, ct.c_void_p, ct.POINTER(ct.c_int64), ct.c_int32, ct.c_void_p, ct.POINTER(ct.c_int64),
+                      ct.c_int32, ct.c_int64, ct.POINTER(ct.c_void_p)]
+        f.restype = ct.c_int
+        mat, matp = _i8(mat)
+        P = BatchParams(matp, n, gap_open, gap_extend, flag, filters, filterd, mask_len, score_size)
+        if table is None:
+            qc, qo = concat(queries)
+            rc, ro = concat(refs)
+            tabp = None
+        else:
+            qs = [q.encode() if isinstance(q, str) else bytes(q) for q in queries]
+            rs = [r.encode() if isinstance(r, str) else bytes(r) for r in refs]
+            qc = np.frombuffer(b"".join(qs) + b"\0", dtype=np.uint8)
+            rc = np.frombuffer(b"".join(rs) + b"\0", dtype=np.uint8)
+            qo = np.zeros(len(qs) + 1, dtype=np.int64); qo[1:] = np.cumsum([len(q) for q in qs])
+            ro = np.zeros(len(rs) + 1, dtype=np.int64); ro[1:] = np.cumsum([len(r) for r in rs])
+            tab = np.ascontiguousarray(table, dtype=np.int8)
+            assert tab.size == 128
+            tabp = tab.ctypes.data_as(ct.POINTER(ct.c_int8))
+        handle = ct.c_void_p()
+        rv = f(self.h, ct.byref(P), tabp, 1 if add_reverse_complement else 0, len(queries), qc.ctypes.data_as(ct.c_void_p),
+               qo.ctypes.data_as(ct.POINTER(ct.c_int64)), len(refs), rc.ctypes.data_as(ct.c_void_p), ro.ctypes.data_as(ct.POINTER(ct.c_int64)),
+               int(min_score), int(max_hits), ct.byref(handle))
+        return _take_hit_set(self.lib, rv, handle, "ssw_group_search_all", max_hits)

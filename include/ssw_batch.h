@@ -126,6 +126,41 @@ int ssw_engine_search(ssw_engine* e, const ssw_batch_params* params, int32_t k, 
                       uint32_t* cigar_pool, int64_t pool_cap, int64_t* pool_used);
 
 /*
+ * Threshold search of the resident queries against the resident references (full grid): EVERY hit, not the k best.  The
+ * size of the answer is known only at the end, so the library allocates it and hands back an opaque set; read it with
+ * ssw_hit_set_view and release it with ssw_hit_set_destroy.
+ *   hit        the rule of ssw_engine_search: status 1, or score1 >= max(min_score, 1)
+ *   output     a sparse matrix in CSR form, one row per resident query (with reverse complements resident, 2 * n_queries
+ *              rows, the reverse complements after the queries): row q's hits are [row_off[q], row_off[q + 1]) of hit_ref
+ *              (the caller's reference index) and hits; row_off has n_rows + 1 entries
+ *   order      within a row, ascending reference index -- so the whole output is in pair order: it is exactly ssw_engine_align
+ *              of the full grid with the same params with the non-hits removed (a caller who wants rank order sorts a row)
+ *   records    field for field what ssw_engine_align returns for that pair; begins and CIGARs (flag & 7) are computed for the
+ *              hits only, into a CIGAR pool the set owns (cigar_off counts words of that pool, at most 2^31 of them)
+ *   max_hits   >= 0; a call that finds more hits returns -2 and no set (it may stop as soon as its running count passes the
+ *              bound: the guard against a low min_score on a grid of 10^8 pairs)
+ * The result does not depend on the path that ran, on how the grid was cut into launch groups or on the number of devices.
+ * Where the grid path runs, the hits of every launch group are counted and compacted on the device and copied back while the
+ * next group computes: no record of a non-hit crosses to the host, and the device holds one launch group's hits at a time.
+ * Which pairs run where is as for ssw_engine_search.  Every failure leaves *out NULL.
+ */
+typedef struct ssw_hit_set ssw_hit_set;
+typedef struct {
+	int32_t n_rows;
+	int64_t n_hits;
+	const int64_t* row_off;            /* n_rows + 1 */
+	const int32_t* hit_ref;            /* n_hits */
+	const ssw_batch_result* hits;      /* n_hits */
+	const uint32_t* cigar_pool;        /* pool_used words (NULL if none) */
+	int64_t pool_used;
+} ssw_hit_view;
+
+int ssw_engine_search_all(ssw_engine* e, const ssw_batch_params* params, int32_t min_score, int64_t max_hits, ssw_hit_set** out);
+/* Pointers into the set, valid until ssw_hit_set_destroy. */
+int ssw_hit_set_view(const ssw_hit_set* s, ssw_hit_view* v);
+void ssw_hit_set_destroy(ssw_hit_set* s);
+
+/*
  * mark_mismatch (ssw.h:157-164; ssw.c:1019-1074) for the CIGARs of a whole batch, on the device: for every record of
  * `results` that carries a CIGAR (words at cigar_pool[cigar_off ...]) the M runs are split into '=' and 'X' runs, soft
  * clips are added for the unaligned ends of the read, and nm[p] (may be NULL) receives the number of mismatching +
@@ -213,6 +248,15 @@ int ssw_group_search(ssw_group* g, const ssw_batch_params* params, const int8_t*
                      int32_t k, int32_t min_score, int32_t* hit_ref, ssw_batch_result* hits, int32_t* n_hits,
                      uint32_t* cigar_pool, int64_t pool_cap, int64_t* pool_used);
 
+/* ssw_engine_search_all over the devices of the group: the queries are cut as for ssw_group_search, every device returns a
+ * set for its block, and the rows are concatenated in query order (with add_reverse_complement the 2 * n_queries rows of
+ * ssw_group_search), which keeps pair order; the CIGAR pools are concatenated (cigar_off re-based).  max_hits bounds the
+ * total.  Results do not depend on the number of devices. */
+int ssw_group_search_all(ssw_group* g, const ssw_batch_params* params, const int8_t* table, int32_t add_reverse_complement,
+                         int32_t n_queries, const void* queries, const int64_t* query_off,
+                         int32_t n_refs, const void* refs, const int64_t* ref_off,
+                         int32_t min_score, int64_t max_hits, ssw_hit_set** out);
+
 /* The same with heap s_align records (ssw_align_batch / _text / _marked over a group); release with align_destroy. */
 int ssw_group_align_batch(ssw_group* g, const ssw_batch_params* params, const int8_t* table, int32_t add_reverse_complement,
                           int32_t n_queries, const void* queries, const int64_t* query_off,
@@ -220,8 +264,8 @@ int ssw_group_align_batch(ssw_group* g, const ssw_batch_params* params, const in
                           int64_t n_pairs, const int32_t* pair_query, const int32_t* pair_ref,
                           s_align** out, int32_t marked, int32_t* nm);
 
-/* Device-time breakdown of the last ssw_engine_align / ssw_engine_search call (CUDA events on the engine's stream), in ms.
- * A search counts its selection kernels in other_launches / resolve_ms. */
+/* Device-time breakdown of the last ssw_engine_align / ssw_engine_search / ssw_engine_search_all call (CUDA events on the
+ * engine's stream), in ms.  A search counts its selection (count and compaction) kernels in other_launches / resolve_ms. */
 typedef struct {
 	float fill_forward_ms;   /* matrix fill kernels, forward pass (incl. byte->word reruns) */
 	float resolve_ms;        /* bookkeeping kernels */
@@ -234,7 +278,7 @@ typedef struct {
 	/* counts of the device-planned grid, exact and known before a kernel runs (0 when no grid was planned) */
 	int64_t grid_cols_planned;   /* group-columns the fill launches sweep: over the warps, groups per warp x the longest reference of the warp */
 	int64_t grid_cols_useful;    /* of these, columns of a group's own reference; useful / planned = the planned sweep efficiency */
-	int64_t leftover_pairs;      /* ssw_engine_search: pairs outside the device-planned grid (general path, selection on the host) */
+	int64_t leftover_pairs;      /* ssw_engine_search(_all): pairs outside the device-planned grid (general path, selection on the host) */
 } ssw_engine_timing;
 int ssw_engine_last_timing(const ssw_engine* e, ssw_engine_timing* t);
 /* Column maxima of the engine's last forward fill launch, for tests: packed s16x2 words (the two alignments of a pair-task),
