@@ -103,6 +103,8 @@ struct SswOptions {
 	int grid_order = 1;             /* "grid_order": 1 = the device-planned grid sweeps the references of a query pair longest first, so that the
 	                                 * groups of a warp end together; 0 = in reference order (measurements) */
 	int grid_max_ref = SSW_GRID_MAX_REF;   /* "grid_max_ref": longer references are not planned on the device (tests) */
+	int64_t grid_tile_refs = 0;     /* "grid_tile_refs": at most this many references per grid tile of a search (0 automatic: tiles only where a
+	                                 * grid has more than 2^31 - 1 pairs or one query pair's scratch exceeds the launch budget; tests, measurements) */
 	int force_inst = -1;            /* "inst" (measurements): use this forward instance whenever it covers the query */
 	int tb_maxbw = SSW_TBP_MAXBW;   /* "tb_maxbw": widest band handled by the shared-memory traceback kernel */
 	int tb_spec = -1;               /* "tb_spec": 1 = band-doubling rounds of a task side by side (speculative kernel), 0 = one after the other, -1 = automatic (small batches) */
@@ -130,6 +132,7 @@ static const SswOptionDef kOptions[] = {
 	{"grid_min", [](SswOptions& o, int64_t v) { o.grid_min_pairs = v < 0 ? 32768 : (int)v; }},
 	{"grid_order", [](SswOptions& o, int64_t v) { o.grid_order = v != 0 ? 1 : 0; }},
 	{"grid_max_ref", [](SswOptions& o, int64_t v) { o.grid_max_ref = v < 1 ? SSW_GRID_MAX_REF : (int)std::min<int64_t>(v, SSW_GRID_MAX_REF); }},
+	{"grid_tile_refs", [](SswOptions& o, int64_t v) { o.grid_tile_refs = v < 0 ? 0 : v; }},
 	{"inst", [](SswOptions& o, int64_t v) { o.force_inst = (int)v; }},       /* index into kInst */
 	{"super", [](SswOptions& o, int64_t v) { o.strip_super = v >= 64 ? (int)(v + 7) / 8 * 8 : SSW_STRIP_SUPER; }},
 	{"tb_spec", [](SswOptions& o, int64_t v) { o.tb_spec = v < 0 ? -1 : (int)v; }},      /* > 1: on, rounds up to that many columns */
@@ -1385,11 +1388,13 @@ struct GridSearch {
 /* Returns 1 when the grid path handled the batch (results filled -- or, with `gs`, the hit table; `redo` lists pairs to re-do
  * by the general path, numbered q * n_r + r), 0 when the batch is not eligible, < 0 on error.
  * An align (`results`) takes the grid as a whole or not at all.  A search (`gs`) takes the queries and the references that
- * qualify one by one and reports them in gs->q_on / r_on; every other pair is left to the caller. */
+ * qualify one by one and reports them in gs->q_on / r_on; every other pair is left to the caller.  A search's references are
+ * cut into grid tiles (contiguous ranges of them), each run as a grid of its own, where the grid has more pairs than 32-bit
+ * pair numbers hold or one query pair's scratch over all references exceeds the launch budget. */
 static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, int64_t n_pairs,
-                       ssw_batch_result* results, std::vector<int32_t>* redo, GridSearch* gs = nullptr)
+                       ssw_batch_result* results, std::vector<int64_t>* redo, GridSearch* gs = nullptr)
 {
-	if (n_pairs != (int64_t)e->n_q * e->n_r || n_pairs < e->opt.grid_min_pairs || n_pairs > 0x7fffffff) return 0;
+	if (n_pairs != (int64_t)e->n_q * e->n_r || n_pairs < e->opt.grid_min_pairs || (!gs && n_pairs > 0x7fffffff)) return 0;
 	if (P.flag != 0 || P.gap_open <= P.gap_extend || e->opt.chunk != 0) return 0;
 	if (!S.has_byte && !S.has_word) return 0;
 	const int word = S.has_byte ? 0 : 1;
@@ -1423,28 +1428,8 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 		if (qt[x].lp != qt[y].lp) return qt[x].lp < qt[y].lp;
 		return x < y;
 	});
-	/* reference tables */
-	std::vector<int64_t> cm_prefix((size_t)n_r), g_off((size_t)n_r);
-	std::vector<int32_t> g_len((size_t)n_r), perm((size_t)n_r);
-	int64_t cm_per_qp = 0;
-	for (int r = 0; r < n_r; ++r) {
-		g_off[r] = e->r_off[rsel[r]]; g_len[r] = e->r_len[rsel[r]]; perm[r] = r;
-		cm_prefix[r] = cm_per_qp; cm_per_qp += ((int64_t)g_len[r] + 3) / 4 * 4;
-	}
-	/* The order in which a query pair's items sweep the references: longest first.  The groups of a warp run until the longest
-	 * of their items is done, so neighbours of equal length waste no steps, and the longest items of a launch start first.
-	 * Stable: references of equal length keep their order (a database of one length is launched exactly as without it). */
-	if (e->opt.grid_order) std::stable_sort(perm.begin(), perm.end(), [&](int32_t x, int32_t y) { return g_len[x] > g_len[y]; });
-	/* planned sweep of one query pair: group-columns of the warps (groups per warp x the warp's longest item) by groups per warp */
-	int64_t cols_useful = 0, cols_planned[3] = {0, 0, 0};                 /* 1, 2, 4 groups per warp */
-	for (int r = 0; r < n_r; ++r) cols_useful += g_len[r];
-	for (int s = 0; s < 3; ++s)
-		for (int r0 = 0; r0 < n_r; r0 += 1 << s) {
-			int32_t longest = 0;
-			for (int r = r0; r < std::min(n_r, r0 + (1 << s)); ++r) longest = std::max(longest, g_len[perm[r]]);
-			cols_planned[s] += (int64_t)longest << s;
-		}
-	/* static tables on the device: [qt][ref_off][ref_len][cm_prefix][perm] */
+	/* static tables on the device: [qt][ref_off][ref_len][cm_prefix][perm]; the reference tables hold one grid tile at a time,
+	 * at most all n_r references */
 	const size_t o_qt = 0, o_roff = o_qt + (sizeof(SswGridQ) * n_q + 255) / 256 * 256, o_rlen = o_roff + (8 * (size_t)n_r + 255) / 256 * 256;
 	const size_t o_cmp = o_rlen + (4 * (size_t)n_r + 255) / 256 * 256, o_perm = o_cmp + (8 * (size_t)n_r + 255) / 256 * 256;
 	const size_t o_qp = o_perm + (4 * (size_t)n_r + 255) / 256 * 256;
@@ -1457,20 +1442,17 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 	if (e->d_grid.ensure(all ? o_soff + 8 * (n_slots + 1) : o_list + 4 * (size_t)redo_cap)) return -1;
 	uint8_t* gb = e->d_grid.as<uint8_t>();
 	SSW_CUDA_OK(cudaMemcpyAsync(gb + o_qt, qt.data(), sizeof(SswGridQ) * n_q, cudaMemcpyHostToDevice, e->stream));
-	SSW_CUDA_OK(cudaMemcpyAsync(gb + o_roff, g_off.data(), 8 * (size_t)n_r, cudaMemcpyHostToDevice, e->stream));
-	SSW_CUDA_OK(cudaMemcpyAsync(gb + o_rlen, g_len.data(), 4 * (size_t)n_r, cudaMemcpyHostToDevice, e->stream));
-	SSW_CUDA_OK(cudaMemcpyAsync(gb + o_cmp, cm_prefix.data(), 8 * (size_t)n_r, cudaMemcpyHostToDevice, e->stream));
-	SSW_CUDA_OK(cudaMemcpyAsync(gb + o_perm, perm.data(), 4 * (size_t)n_r, cudaMemcpyHostToDevice, e->stream));
 	SSW_CUDA_OK(cudaMemsetAsync(gb + o_cnt, 0, 256, e->stream));
-	/* search: [hits n_q*k][hit_ref n_q*k][n_hits n_q], every row written by the selection kernel of its query */
+	/* search: [hits n_q*k][hit_ref n_q*k][n_hits n_q], every row written by the selection kernel of its query (first grid tile)
+	 * or merged from a table of the same layout at o_tile (later tiles) */
 	const size_t o_href = sizeof(ssw_batch_result) * (size_t)n_q * (gs ? gs->k : 0), o_nh = o_href + 4 * (size_t)n_q * (gs ? gs->k : 0);
+	const size_t o_tile = o_nh + 4 * (size_t)n_q;
 	if (all) {
 		/* the hits of one launch group at a time, in e->d_hits (grown per group) */
-	} else if (gs ? e->d_hits.ensure(o_nh + 4 * (size_t)n_q) : e->d_out.ensure(sizeof(ssw_batch_result) * (size_t)n_pairs)) return -1;
-	if (gs && !all) SSW_CUDA_OK(cudaMemsetAsync(e->d_hits.as<uint8_t>() + o_nh, 0, 4 * (size_t)n_q, e->stream));   /* queries off the grid: no hits here */
+	} else if (gs ? e->d_hits.ensure(o_tile) : e->d_out.ensure(sizeof(ssw_batch_result) * (size_t)n_pairs)) return -1;
 	/* threshold search: the group whose hits are still on the device, and a copy that brings them to gs->rows.  The device buffer
 	 * is written by the next group's compaction only after this copy has returned, so one buffer serves every group. */
-	struct HitGroup { int64_t n = 0; std::vector<int64_t> off; std::vector<int32_t> q; cudaEvent_t ev = nullptr; };
+	struct HitGroup { int64_t n = 0; std::vector<int64_t> off; std::vector<int32_t> q; int32_t r_lo = 0; cudaEvent_t ev = nullptr; };
 	HitGroup pend;
 	int64_t grid_hits = 0;
 	if (all) gs->rows.assign((size_t)n_q, std::vector<SearchHit>());
@@ -1486,7 +1468,7 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 		for (size_t s = 0; s < pend.q.size(); ++s) {
 			if (pend.q[s] < 0) continue;
 			std::vector<SearchHit>& row = gs->rows[pend.q[s]];
-			for (int64_t i = pend.off[s]; i < pend.off[s + 1]; ++i) row.push_back(SearchHit{rsel[hr[i]], h[i]});   /* rsel ascending: order kept */
+			for (int64_t i = pend.off[s]; i < pend.off[s + 1]; ++i) row.push_back(SearchHit{rsel[pend.r_lo + hr[i]], h[i]});   /* rsel ascending: order kept */
 		}
 		pend = HitGroup();
 		return 0;
@@ -1495,161 +1477,249 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 	const size_t free_b = ssw_free_device_bytes();
 	const size_t budget = std::max<size_t>((size_t)256 << 20, ssw_budget_share(free_b + e->d_colmax.cap + e->d_items.cap + e->d_alns.cap + e->d_res.cap));
 	tr.lap("grid: tables");
+	/* Grid tiles of a search: the longest runs of references (in rsel order) with at most 2^31 - 1 pairs numbered q * n_rt + r
+	 * (q: any resident query) and one query pair's scratch within the budget -- one tile wherever both hold for all references.
+	 * An align is never cut. */
+	std::vector<int32_t> tile_lo(1, 0);
+	if (gs) {
+		std::vector<int> per_ctas;                   /* items per CTA of the instances of the grid's queries */
+		for (int32_t q : order) {
+			const int c = fill_items_per_cta(q_inst[q], P.n);
+			if (std::find(per_ctas.begin(), per_ctas.end(), c) == per_ctas.end()) per_ctas.push_back(c);
+		}
+		auto qp_bytes = [&](int64_t nr, int64_t cm_words) {   /* per_qp of the launch groups below, for the widest instance */
+			size_t b = 0;
+			for (int c : per_ctas)
+				b = std::max(b, (size_t)cm_words * 4 + (size_t)((nr + c - 1) / c * c) * (sizeof(SswItem) + sizeof(SswItemBest)) + (size_t)nr * 2 * (sizeof(SswAlnDesc) + sizeof(SswFillResult)));
+			return b;
+		};
+		int64_t cap = 0x7fffffff / n_q;
+		if (e->opt.grid_tile_refs > 0) cap = std::min(cap, e->opt.grid_tile_refs);
+		int64_t cm_words = 0;
+		for (int r = 0; r < n_r; ++r) {
+			const int64_t w = ((int64_t)e->r_len[rsel[r]] + 3) / 4 * 4, n = r - tile_lo.back();
+			if (n > 0 && (n + 1 > cap || qp_bytes(n + 1, cm_words + w) > budget)) { tile_lo.push_back(r); cm_words = 0; }
+			cm_words += w;
+		}
+	}
+	tile_lo.push_back(n_r);
+	const size_t n_tiles = tile_lo.size() - 1;
+	if (gs && !all) {
+		if (n_tiles > 1 && e->d_hits.ensure(o_tile + o_nh + 4 * (size_t)n_q)) return -1;
+		SSW_CUDA_OK(cudaMemsetAsync(e->d_hits.as<uint8_t>() + o_nh, 0, 4 * (size_t)n_q, e->stream));   /* queries off the grid: no hits here */
+	}
+	/* The redo list holds the pairs of one tile, numbered on its tables; after each tile they are mapped to the caller's numbers.
+	 * More than the list holds in any tile: the whole call goes through the general path (the overflows cannot be found). */
+	bool redo_over = false;
+	auto take_redo = [&](int32_t r_lo, int32_t n_rt) -> int {
+		int32_t n_redo = 0;
+		SSW_CUDA_OK(cudaMemcpyAsync(&n_redo, gb + o_cnt, 4, cudaMemcpyDeviceToHost, e->stream));
+		SSW_CUDA_OK(cudaStreamSynchronize(e->stream));
+		if (n_redo > redo_cap) { redo_over = true; return 0; }
+		if (n_redo) {
+			std::vector<int32_t> list((size_t)n_redo);
+			SSW_CUDA_OK(cudaMemcpy(list.data(), gb + o_list, 4 * (size_t)n_redo, cudaMemcpyDeviceToHost));
+			for (int32_t p : list) redo->push_back((int64_t)(p / n_rt) * n_r_all + rsel[r_lo + p % n_rt]);
+		}
+		return 0;
+	};
 	struct GridGroup { cudaEvent_t ev; int32_t q_lo, q_n; bool contiguous; };
 	std::vector<GridGroup> groups;
 	/* Late arming of the best-cell bookkeeping (ssw_fill.cuh): rows are recorded in the last arm_tail columns of every
 	 * reference only.  Automatic for protein-like alphabets, where the running maximum grows with every column and the
 	 * maximum of a pair lies near the end of the reference; a small pilot group goes first and the rest of the grid is
-	 * armed from column 0 again if more than 0.2 % of the pilot's pairs had to be re-done. */
+	 * armed from column 0 again if more than 0.2 % of the pilot's pairs had to be re-done.  The pilot runs in the first tile. */
 	bool arm_on = e->opt.grid_arm > 0 || (e->opt.grid_arm < 0 && P.n > 8 && e->grid_arm_ok);
 	bool pilot_pending = arm_on && e->opt.grid_arm < 0;
 	int64_t pilot_pairs = 0;
-	size_t k = 0;
-	while (k < order.size()) {
-		const int inst = q_inst[order[k]];
-		const int per_cta = fill_items_per_cta(inst, P.n);
-		const int n_r_pad = (n_r + per_cta - 1) / per_cta * per_cta;
-		/* query pairs of this launch: same instance, bounded by memory */
-		const size_t per_qp = (size_t)cm_per_qp * 4 + (size_t)n_r_pad * (sizeof(SswItem) + sizeof(SswItemBest)) + (size_t)n_r * 2 * (sizeof(SswAlnDesc) + sizeof(SswFillResult));
-		size_t max_qp = std::max<size_t>(1, budget / per_qp);
-		/* large grids: several launch groups even when memory would allow one, so that the records of a finished group are
-		 * copied to the host while the next group computes (115 MB of records per million pairs) */
-		if ((int64_t)n_qe * n_r >= e->opt.grid_split_pairs)
-			max_qp = std::min<size_t>(max_qp, std::max<size_t>((size_t)std::max(e->opt.grid_group_qp, 1), ((size_t)n_qe / 2 + 7) / 8));
-		if (pilot_pending && (size_t)n_qe / 2 >= 16) max_qp = std::min<size_t>(max_qp, std::max<size_t>(2, (size_t)n_qe / 64));   /* the pilot: 1/32 of the queries */
-		std::vector<int2> qps;
-		const size_t k_first = k;
-		while (k < order.size() && q_inst[order[k]] == inst && qps.size() < max_qp) {
-			int2 pr = make_int2(order[k], -1);
-			++k;
-			if (k < order.size() && q_inst[order[k]] == inst) { pr.y = order[k]; ++k; }
-			qps.push_back(pr);
+	for (size_t t = 0; t < n_tiles; ++t) {
+		const int32_t r_lo = tile_lo[t], n_rt = tile_lo[t + 1] - r_lo;
+		/* the tile's reference tables: its references numbered 0 .. n_rt - 1 */
+		std::vector<int64_t> cm_prefix((size_t)n_rt), g_off((size_t)n_rt);
+		std::vector<int32_t> g_len((size_t)n_rt), perm((size_t)n_rt);
+		int64_t cm_per_qp = 0;
+		for (int r = 0; r < n_rt; ++r) {
+			g_off[r] = e->r_off[rsel[r_lo + r]]; g_len[r] = e->r_len[rsel[r_lo + r]]; perm[r] = r;
+			cm_prefix[r] = cm_per_qp; cm_per_qp += ((int64_t)g_len[r] + 3) / 4 * 4;
 		}
-		SswGridArgs A;
-		A.n_qp = (int32_t)qps.size(); A.n_r = n_r; A.n_r_pad = n_r_pad; A.word = word; A.limit = limit; A.cm_words_per_qp = cm_per_qp;
-		A.arm_tail = 0;
-		if (arm_on) {
-			int lp_max = 0;
-			for (const int2& pr : qps) { lp_max = std::max(lp_max, qt[pr.x].lp); if (pr.y >= 0) lp_max = std::max(lp_max, qt[pr.y].lp); }
-			A.arm_tail = e->opt.grid_arm > 0 ? e->opt.grid_arm : lp_max / 4 + 64;
-		}
-		const int64_t n_items = (int64_t)A.n_qp * n_r_pad, n_desc = (int64_t)A.n_qp * n_r * 2;
-		if (n_items > 0x7fffffff || n_desc > 0x7fffffff) return 0;
-		if (e->d_items.ensure(sizeof(SswItem) * (size_t)n_items)) return -1;
-		if (e->d_bests.ensure(sizeof(SswItemBest) * (size_t)n_items)) return -1;
-		if (e->d_alns.ensure(sizeof(SswAlnDesc) * (size_t)n_desc)) return -1;
-		if (e->d_res.ensure(sizeof(SswFillResult) * (size_t)n_desc)) return -1;
-		if (e->d_colmax.ensure((size_t)A.n_qp * (size_t)cm_per_qp * 4 + 64)) return -1;
-		SSW_CUDA_OK(cudaMemcpyAsync(gb + o_qp, qps.data(), sizeof(int2) * qps.size(), cudaMemcpyHostToDevice, e->stream));
-		e->laps.start(e->stream);
-		ssw_launch(ssw_grid_plan_kernel, dim3((unsigned)((n_items + 255) / 256)), dim3(256), 0, e->stream, A,
-		           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
-		           (const int64_t*)reinterpret_cast<int64_t*>(gb + o_roff), (const int32_t*)reinterpret_cast<int32_t*>(gb + o_rlen),
-		           (const int64_t*)reinterpret_cast<int64_t*>(gb + o_cmp), (const int32_t*)reinterpret_cast<int32_t*>(gb + o_perm),
-		           e->d_items.as<SswItem>(), e->d_alns.as<SswAlnDesc>());
-		SSW_CUDA_OK(cudaGetLastError());
-		e->laps.stop(e->stream, &e->timing.resolve_ms);
-		e->timing.other_launches += 1;
-		/* fill (items are already on the device) */
-		{
+		/* The order in which a query pair's items sweep the references: longest first.  The groups of a warp run until the longest
+		 * of their items is done, so neighbours of equal length waste no steps, and the longest items of a launch start first.
+		 * Stable: references of equal length keep their order (a database of one length is launched exactly as without it). */
+		if (e->opt.grid_order) std::stable_sort(perm.begin(), perm.end(), [&](int32_t x, int32_t y) { return g_len[x] > g_len[y]; });
+		/* planned sweep of one query pair: group-columns of the warps (groups per warp x the warp's longest item) by groups per warp */
+		int64_t cols_useful = 0, cols_planned[3] = {0, 0, 0};                 /* 1, 2, 4 groups per warp */
+		for (int r = 0; r < n_rt; ++r) cols_useful += g_len[r];
+		for (int s = 0; s < 3; ++s)
+			for (int r0 = 0; r0 < n_rt; r0 += 1 << s) {
+				int32_t longest = 0;
+				for (int r = r0; r < std::min(n_rt, r0 + (1 << s)); ++r) longest = std::max(longest, g_len[perm[r]]);
+				cols_planned[s] += (int64_t)longest << s;
+			}
+		SSW_CUDA_OK(cudaMemcpyAsync(gb + o_roff, g_off.data(), 8 * (size_t)n_rt, cudaMemcpyHostToDevice, e->stream));
+		SSW_CUDA_OK(cudaMemcpyAsync(gb + o_rlen, g_len.data(), 4 * (size_t)n_rt, cudaMemcpyHostToDevice, e->stream));
+		SSW_CUDA_OK(cudaMemcpyAsync(gb + o_cmp, cm_prefix.data(), 8 * (size_t)n_rt, cudaMemcpyHostToDevice, e->stream));
+		SSW_CUDA_OK(cudaMemcpyAsync(gb + o_perm, perm.data(), 4 * (size_t)n_rt, cudaMemcpyHostToDevice, e->stream));
+		size_t k = 0;
+		while (k < order.size()) {
+			const int inst = q_inst[order[k]];
+			const int per_cta = fill_items_per_cta(inst, P.n);
+			const int n_r_pad = (n_rt + per_cta - 1) / per_cta * per_cta;
+			/* query pairs of this launch: same instance, bounded by memory */
+			const size_t per_qp = (size_t)cm_per_qp * 4 + (size_t)n_r_pad * (sizeof(SswItem) + sizeof(SswItemBest)) + (size_t)n_rt * 2 * (sizeof(SswAlnDesc) + sizeof(SswFillResult));
+			size_t max_qp = std::max<size_t>(1, budget / per_qp);
+			/* large grids: several launch groups even when memory would allow one, so that the records of a finished group are
+			 * copied to the host while the next group computes (115 MB of records per million pairs) */
+			if ((int64_t)n_qe * n_r >= e->opt.grid_split_pairs)
+				max_qp = std::min<size_t>(max_qp, std::max<size_t>((size_t)std::max(e->opt.grid_group_qp, 1), ((size_t)n_qe / 2 + 7) / 8));
+			if (pilot_pending && (size_t)n_qe / 2 >= 16) max_qp = std::min<size_t>(max_qp, std::max<size_t>(2, (size_t)n_qe / 64));   /* the pilot: 1/32 of the queries */
+			std::vector<int2> qps;
+			const size_t k_first = k;
+			while (k < order.size() && q_inst[order[k]] == inst && qps.size() < max_qp) {
+				int2 pr = make_int2(order[k], -1);
+				++k;
+				if (k < order.size() && q_inst[order[k]] == inst) { pr.y = order[k]; ++k; }
+				qps.push_back(pr);
+			}
+			SswGridArgs A;
+			A.n_qp = (int32_t)qps.size(); A.n_r = n_rt; A.n_r_pad = n_r_pad; A.word = word; A.limit = limit; A.cm_words_per_qp = cm_per_qp;
+			A.arm_tail = 0;
+			if (arm_on) {
+				int lp_max = 0;
+				for (const int2& pr : qps) { lp_max = std::max(lp_max, qt[pr.x].lp); if (pr.y >= 0) lp_max = std::max(lp_max, qt[pr.y].lp); }
+				A.arm_tail = e->opt.grid_arm > 0 ? e->opt.grid_arm : lp_max / 4 + 64;
+			}
+			const int64_t n_items = (int64_t)A.n_qp * n_r_pad, n_desc = (int64_t)A.n_qp * n_rt * 2;
+			if (n_items > 0x7fffffff || n_desc > 0x7fffffff) return 0;
+			if (e->d_items.ensure(sizeof(SswItem) * (size_t)n_items)) return -1;
+			if (e->d_bests.ensure(sizeof(SswItemBest) * (size_t)n_items)) return -1;
+			if (e->d_alns.ensure(sizeof(SswAlnDesc) * (size_t)n_desc)) return -1;
+			if (e->d_res.ensure(sizeof(SswFillResult) * (size_t)n_desc)) return -1;
+			if (e->d_colmax.ensure((size_t)A.n_qp * (size_t)cm_per_qp * 4 + 64)) return -1;
+			SSW_CUDA_OK(cudaMemcpyAsync(gb + o_qp, qps.data(), sizeof(int2) * qps.size(), cudaMemcpyHostToDevice, e->stream));
 			e->laps.start(e->stream);
-			FillPtrs fp = {e->d_items.as<SswItem>(), e->d_colmax.as<uint32_t>(), e->d_bests.as<SswItemBest>()};
-			fp.arm = A.arm_tail > 0;
-			const int rc = dispatch_fill(e, inst, fp, (int)n_items, +1, 1, 1, P);
-			if (rc) return rc < 0 ? rc : -1;
-			e->laps.stop(e->stream, &e->timing.fill_forward_ms);
-			e->timing.fill_forward_launches += 1;
-			e->timing.cells_forward += (int64_t)A.n_qp * (cm_per_qp) * inst_rows(inst) * 2;
-			e->timing.grid_cols_useful += (int64_t)A.n_qp * cols_useful;
-			e->timing.grid_cols_planned += (int64_t)A.n_qp * cols_planned[kInst[inst].G == 32 ? 0 : kInst[inst].G == 16 ? 1 : 2];
-		}
-		e->laps.start(e->stream);
-		{
-			const int per = SSW_RESOLVE_THREADS / 32;
-			ssw_launch(ssw_resolve_kernel<true>, dim3((unsigned)((n_desc + per - 1) / per)), dim3(SSW_RESOLVE_THREADS), 0, e->stream,
-			           (const SswAlnDesc*)e->d_alns.as<SswAlnDesc>(), (int)n_desc, (const SswItemBest*)e->d_bests.as<SswItemBest>(),
-			           (const uint32_t*)e->d_colmax.as<uint32_t>(), e->d_res.as<SswFillResult>());
-			if (!gs)
-				ssw_launch(ssw_grid_emit_kernel, dim3((unsigned)((n_desc + 255) / 256)), dim3(256), 0, e->stream, A,
-				           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
-				           (const SswFillResult*)e->d_res.as<SswFillResult>(), e->d_out.as<ssw_batch_result>(),
-				           reinterpret_cast<int32_t*>(gb + o_list), reinterpret_cast<int32_t*>(gb + o_cnt), redo_cap);
-			else if (all)
-				ssw_launch(ssw_grid_count_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream, A,
-				           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
-				           (const SswFillResult*)e->d_res.as<SswFillResult>(), gs->min_score, reinterpret_cast<int32_t*>(gb + o_scnt),
-				           reinterpret_cast<int32_t*>(gb + o_list), reinterpret_cast<int32_t*>(gb + o_cnt), redo_cap);
-			else {
-				uint8_t* hb = e->d_hits.as<uint8_t>();
-				ssw_launch(ssw_grid_select_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream, A,
-				           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
-				           (const SswFillResult*)e->d_res.as<SswFillResult>(), gs->k, gs->min_score,
-				           reinterpret_cast<int32_t*>(hb + o_href), reinterpret_cast<ssw_batch_result*>(hb), reinterpret_cast<int32_t*>(hb + o_nh),
-				           reinterpret_cast<int32_t*>(gb + o_list), reinterpret_cast<int32_t*>(gb + o_cnt), redo_cap);
-			}
+			ssw_launch(ssw_grid_plan_kernel, dim3((unsigned)((n_items + 255) / 256)), dim3(256), 0, e->stream, A,
+			           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
+			           (const int64_t*)reinterpret_cast<int64_t*>(gb + o_roff), (const int32_t*)reinterpret_cast<int32_t*>(gb + o_rlen),
+			           (const int64_t*)reinterpret_cast<int64_t*>(gb + o_cmp), (const int32_t*)reinterpret_cast<int32_t*>(gb + o_perm),
+			           e->d_items.as<SswItem>(), e->d_alns.as<SswAlnDesc>());
 			SSW_CUDA_OK(cudaGetLastError());
-		}
-		e->laps.stop(e->stream, &e->timing.resolve_ms);
-		e->timing.other_launches += 2;
-		/* the group's records are final once its emit kernel has run: remember the event and, when the group's queries are a
-		 * contiguous ascending range (equal-length queries: `order` is the identity), the slice of records they own */
-		GridGroup gg;
-		if (e->grid_event(groups.size(), &gg.ev)) return -1;
-		SSW_CUDA_OK(cudaEventRecord(gg.ev, e->stream));
-		gg.q_lo = order[k_first]; gg.q_n = (int32_t)(k - k_first); gg.contiguous = true;
-		for (size_t i = k_first; i < k; ++i) if (order[i] != gg.q_lo + (int32_t)(i - k_first)) gg.contiguous = false;
-		groups.push_back(gg);
-		if (pilot_pending) {
-			/* how many of the pilot's pairs must be re-done?  (byte overflows count too: either way the grid path does not pay off) */
-			pilot_pending = false;
-			int32_t n_now = 0;
-			SSW_CUDA_OK(cudaMemcpyAsync(&n_now, gb + o_cnt, 4, cudaMemcpyDeviceToHost, e->stream));
-			SSW_CUDA_OK(cudaStreamSynchronize(e->stream));
-			pilot_pairs = (int64_t)A.n_qp * 2 * n_r;
-			if ((int64_t)n_now * 500 > pilot_pairs) {    /* a re-done pair costs ~400x what arming saves per pair */
-				/* arming does not pay for these sequences: forget the pilot (its re-do list too) and run its queries again,
-				 * armed from column 0, as the first regular group -- 1/32 of the grid is computed twice, nothing goes through
-				 * the general path */
-				arm_on = false; e->grid_arm_ok = false;
-				SSW_CUDA_OK(cudaMemsetAsync(gb + o_cnt, 0, 256, e->stream));
-				groups.pop_back();
-				k = k_first;
-				tr.lap("grid: pilot group rejected");
-				continue;
-			}
-		}
-		if (all) {
-			/* the previous group's hits come back while this group computes; then this group's counts, the one synchronisation
-			 * per group, and its compaction at their prefix */
-			if (flush_hits()) return -1;
-			HitGroup hg;
-			std::vector<int32_t> sn((size_t)2 * A.n_qp);
-			SSW_CUDA_OK(cudaMemcpyAsync(sn.data(), gb + o_scnt, 4 * sn.size(), cudaMemcpyDeviceToHost, e->stream));
-			SSW_CUDA_OK(cudaStreamSynchronize(e->stream));
-			hg.off.assign(sn.size() + 1, 0); hg.q.resize(sn.size());
-			for (size_t s = 0; s < sn.size(); ++s) { hg.q[s] = s & 1 ? qps[s / 2].y : qps[s / 2].x; hg.off[s + 1] = hg.off[s] + sn[s]; }
-			hg.n = hg.off.back();
-			grid_hits += hg.n;
-			if (grid_hits > gs->max_hits) return -2;
-			if (hg.n > 0) {
-				const size_t o_ref = (sizeof(ssw_batch_result) * (size_t)hg.n + 255) / 256 * 256;
-				if (e->d_hits.ensure(o_ref + 4 * (size_t)hg.n)) return -1;
-				uint8_t* hb = e->d_hits.as<uint8_t>();
-				SSW_CUDA_OK(cudaMemcpyAsync(gb + o_soff, hg.off.data(), 8 * hg.off.size(), cudaMemcpyHostToDevice, e->stream));
+			e->laps.stop(e->stream, &e->timing.resolve_ms);
+			e->timing.other_launches += 1;
+			/* fill (items are already on the device) */
+			{
 				e->laps.start(e->stream);
-				ssw_launch(ssw_grid_compact_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream, A,
-				           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
-				           (const SswFillResult*)e->d_res.as<SswFillResult>(), gs->min_score, (const int64_t*)reinterpret_cast<int64_t*>(gb + o_soff),
-				           reinterpret_cast<int32_t*>(hb + o_ref), reinterpret_cast<ssw_batch_result*>(hb));
-				SSW_CUDA_OK(cudaGetLastError());
-				e->laps.stop(e->stream, &e->timing.resolve_ms);
-				e->timing.other_launches += 1;
-				hg.ev = groups.back().ev;
-				SSW_CUDA_OK(cudaEventRecord(hg.ev, e->stream));
+				FillPtrs fp = {e->d_items.as<SswItem>(), e->d_colmax.as<uint32_t>(), e->d_bests.as<SswItemBest>()};
+				fp.arm = A.arm_tail > 0;
+				const int rc = dispatch_fill(e, inst, fp, (int)n_items, +1, 1, 1, P);
+				if (rc) return rc < 0 ? rc : -1;
+				e->laps.stop(e->stream, &e->timing.fill_forward_ms);
+				e->timing.fill_forward_launches += 1;
+				e->timing.cells_forward += (int64_t)A.n_qp * (cm_per_qp) * inst_rows(inst) * 2;
+				e->timing.grid_cols_useful += (int64_t)A.n_qp * cols_useful;
+				e->timing.grid_cols_planned += (int64_t)A.n_qp * cols_planned[kInst[inst].G == 32 ? 0 : kInst[inst].G == 16 ? 1 : 2];
 			}
-			pend = std::move(hg);
+			e->laps.start(e->stream);
+			{
+				const int per = SSW_RESOLVE_THREADS / 32;
+				ssw_launch(ssw_resolve_kernel<true>, dim3((unsigned)((n_desc + per - 1) / per)), dim3(SSW_RESOLVE_THREADS), 0, e->stream,
+				           (const SswAlnDesc*)e->d_alns.as<SswAlnDesc>(), (int)n_desc, (const SswItemBest*)e->d_bests.as<SswItemBest>(),
+				           (const uint32_t*)e->d_colmax.as<uint32_t>(), e->d_res.as<SswFillResult>());
+				if (!gs)
+					ssw_launch(ssw_grid_emit_kernel, dim3((unsigned)((n_desc + 255) / 256)), dim3(256), 0, e->stream, A,
+					           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
+					           (const SswFillResult*)e->d_res.as<SswFillResult>(), e->d_out.as<ssw_batch_result>(),
+					           reinterpret_cast<int32_t*>(gb + o_list), reinterpret_cast<int32_t*>(gb + o_cnt), redo_cap);
+				else if (all)
+					ssw_launch(ssw_grid_count_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream, A,
+					           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
+					           (const SswFillResult*)e->d_res.as<SswFillResult>(), gs->min_score, reinterpret_cast<int32_t*>(gb + o_scnt),
+					           reinterpret_cast<int32_t*>(gb + o_list), reinterpret_cast<int32_t*>(gb + o_cnt), redo_cap);
+				else {
+					/* the first tile selects into the running table; a later tile into the tile table, merged into the running one */
+					uint8_t* hb = e->d_hits.as<uint8_t>(), *tb = hb + (t ? o_tile : 0);
+					ssw_launch(ssw_grid_select_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream, A,
+					           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
+					           (const SswFillResult*)e->d_res.as<SswFillResult>(), gs->k, gs->min_score,
+					           reinterpret_cast<int32_t*>(tb + o_href), reinterpret_cast<ssw_batch_result*>(tb), reinterpret_cast<int32_t*>(tb + o_nh),
+					           reinterpret_cast<int32_t*>(gb + o_list), reinterpret_cast<int32_t*>(gb + o_cnt), redo_cap);
+					if (t) {
+						ssw_launch(ssw_grid_merge_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream,
+						           (const int2*)reinterpret_cast<int2*>(gb + o_qp), gs->k, r_lo,
+						           reinterpret_cast<int32_t*>(hb + o_href), reinterpret_cast<ssw_batch_result*>(hb), reinterpret_cast<int32_t*>(hb + o_nh),
+						           (const int32_t*)reinterpret_cast<int32_t*>(tb + o_href), (const ssw_batch_result*)reinterpret_cast<ssw_batch_result*>(tb),
+						           (const int32_t*)reinterpret_cast<int32_t*>(tb + o_nh));
+						e->timing.other_launches += 1;
+					}
+				}
+				SSW_CUDA_OK(cudaGetLastError());
+			}
+			e->laps.stop(e->stream, &e->timing.resolve_ms);
+			e->timing.other_launches += 2;
+			/* the group's records are final once its emit kernel has run: remember the event and, when the group's queries are a
+			 * contiguous ascending range (equal-length queries: `order` is the identity), the slice of records they own */
+			GridGroup gg;
+			if (e->grid_event(groups.size(), &gg.ev)) return -1;
+			SSW_CUDA_OK(cudaEventRecord(gg.ev, e->stream));
+			gg.q_lo = order[k_first]; gg.q_n = (int32_t)(k - k_first); gg.contiguous = true;
+			for (size_t i = k_first; i < k; ++i) if (order[i] != gg.q_lo + (int32_t)(i - k_first)) gg.contiguous = false;
+			groups.push_back(gg);
+			if (pilot_pending) {
+				/* how many of the pilot's pairs must be re-done?  (byte overflows count too: either way the grid path does not pay off) */
+				pilot_pending = false;
+				int32_t n_now = 0;
+				SSW_CUDA_OK(cudaMemcpyAsync(&n_now, gb + o_cnt, 4, cudaMemcpyDeviceToHost, e->stream));
+				SSW_CUDA_OK(cudaStreamSynchronize(e->stream));
+				pilot_pairs = (int64_t)A.n_qp * 2 * n_rt;
+				if ((int64_t)n_now * 500 > pilot_pairs) {    /* a re-done pair costs ~400x what arming saves per pair */
+					/* arming does not pay for these sequences: forget the pilot (its re-do list too) and run its queries again,
+					 * armed from column 0, as the first regular group -- 1/32 of the grid is computed twice, nothing goes through
+					 * the general path */
+					arm_on = false; e->grid_arm_ok = false;
+					SSW_CUDA_OK(cudaMemsetAsync(gb + o_cnt, 0, 256, e->stream));
+					groups.pop_back();
+					k = k_first;
+					tr.lap("grid: pilot group rejected");
+					continue;
+				}
+			}
+			if (all) {
+				/* the previous group's hits come back while this group computes; then this group's counts, the one synchronisation
+				 * per group, and its compaction at their prefix */
+				if (flush_hits()) return -1;
+				HitGroup hg;
+				std::vector<int32_t> sn((size_t)2 * A.n_qp);
+				SSW_CUDA_OK(cudaMemcpyAsync(sn.data(), gb + o_scnt, 4 * sn.size(), cudaMemcpyDeviceToHost, e->stream));
+				SSW_CUDA_OK(cudaStreamSynchronize(e->stream));
+				hg.off.assign(sn.size() + 1, 0); hg.q.resize(sn.size()); hg.r_lo = r_lo;
+				for (size_t s = 0; s < sn.size(); ++s) { hg.q[s] = s & 1 ? qps[s / 2].y : qps[s / 2].x; hg.off[s + 1] = hg.off[s] + sn[s]; }
+				hg.n = hg.off.back();
+				grid_hits += hg.n;
+				if (grid_hits > gs->max_hits) return -2;
+				if (hg.n > 0) {
+					const size_t o_ref = (sizeof(ssw_batch_result) * (size_t)hg.n + 255) / 256 * 256;
+					if (e->d_hits.ensure(o_ref + 4 * (size_t)hg.n)) return -1;
+					uint8_t* hb = e->d_hits.as<uint8_t>();
+					SSW_CUDA_OK(cudaMemcpyAsync(gb + o_soff, hg.off.data(), 8 * hg.off.size(), cudaMemcpyHostToDevice, e->stream));
+					e->laps.start(e->stream);
+					ssw_launch(ssw_grid_compact_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream, A,
+					           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
+					           (const SswFillResult*)e->d_res.as<SswFillResult>(), gs->min_score, (const int64_t*)reinterpret_cast<int64_t*>(gb + o_soff),
+					           reinterpret_cast<int32_t*>(hb + o_ref), reinterpret_cast<ssw_batch_result*>(hb));
+					SSW_CUDA_OK(cudaGetLastError());
+					e->laps.stop(e->stream, &e->timing.resolve_ms);
+					e->timing.other_launches += 1;
+					hg.ev = groups.back().ev;
+					SSW_CUDA_OK(cudaEventRecord(hg.ev, e->stream));
+				}
+				pend = std::move(hg);
+			}
+			tr.lap("grid: launch group");
 		}
-		tr.lap("grid: launch group");
+		if (t + 1 < n_tiles) {
+			if (take_redo(r_lo, n_rt)) return -1;
+			if (redo_over) return 0;
+			SSW_CUDA_OK(cudaMemsetAsync(gb + o_cnt, 0, 256, e->stream));
+		}
 	}
 	/* every launch is queued; bring the records back group by group on the copy stream while later groups still compute */
 	bool all_contiguous = !groups.empty();
@@ -1679,18 +1749,9 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 			if (e->staged.copy(results + first, e->d_out.as<ssw_batch_result>() + first, sizeof(ssw_batch_result) * cnt, e->side[0])) return -1;
 		}
 	} else if (e->staged.copy(results, e->d_out.p, sizeof(ssw_batch_result) * (size_t)n_pairs, e->stream)) return -1;
-	int32_t n_redo = 0;
-	SSW_CUDA_OK(cudaMemcpyAsync(&n_redo, gb + o_cnt, 4, cudaMemcpyDeviceToHost, e->stream));
-	SSW_CUDA_OK(cudaStreamSynchronize(e->stream));
-	if (n_redo > redo_cap) {                     /* more overflows than the list holds: find them by scanning is not possible -> general path */
-		return 0;
-	}
-	redo->resize((size_t)n_redo);
-	if (n_redo) {
-		SSW_CUDA_OK(cudaMemcpy(redo->data(), gb + o_list, 4 * (size_t)n_redo, cudaMemcpyDeviceToHost));
-		for (int32_t& p : *redo) p = p / n_r * n_r_all + rsel[p % n_r];          /* the device numbers the pairs of its own tables */
-		std::sort(redo->begin(), redo->end());
-	}
+	if (take_redo(tile_lo[n_tiles - 1], n_r - tile_lo[n_tiles - 1])) return -1;
+	if (redo_over) return 0;
+	std::sort(redo->begin(), redo->end());
 	tr.lap("grid: results d2h");
 	return 1;
 }
@@ -1988,14 +2049,14 @@ static int engine_align_impl(ssw_engine* e, const ssw_batch_params* params,
 			return 0;
 		}
 	}
-	std::vector<int32_t> redo;
+	std::vector<int64_t> redo;
 	const int grid = pair_query ? 0 : grid_scores(e, P, S, n_pairs, results, &redo);
 	if (grid < 0) return grid;
 	if (grid == 1) {
 		/* the device-planned grid handled everything except byte overflows: those pairs go through the general path */
 		if (!redo.empty()) {
 			std::vector<int32_t> pq(redo.size()), pr(redo.size());
-			for (size_t i = 0; i < redo.size(); ++i) { pq[i] = redo[i] / e->n_r; pr[i] = redo[i] % e->n_r; }
+			for (size_t i = 0; i < redo.size(); ++i) { pq[i] = (int32_t)(redo[i] / e->n_r); pr[i] = (int32_t)(redo[i] % e->n_r); }
 			std::vector<ssw_batch_result> sub(redo.size());
 			const ssw_engine_timing keep = e->timing;
 			rc = align_general(e, P, S, (int64_t)redo.size(), pq.data(), pr.data(), sub.data(), cigar_pool, pool_cap, pool_used);
@@ -2088,7 +2149,7 @@ static int search_rows(ssw_engine* e, const ssw_batch_params& P, int32_t keep, i
 	};
 	GridSearch gs;
 	gs.k = keep; gs.min_score = thr; gs.max_hits = max_hits;
-	std::vector<int32_t> redo;
+	std::vector<int64_t> redo;
 	int rc = grid_scores(e, P0, S, (int64_t)n_q * n_r, nullptr, &redo, &gs);
 	if (rc < 0) return rc;
 	if (rc == 1) {
@@ -2103,7 +2164,7 @@ static int search_rows(ssw_engine* e, const ssw_batch_params& P, int32_t keep, i
 		 * and the re-done pairs, whatever the reason of the re-do */
 		if (!redo.empty()) {
 			std::vector<int32_t> pq(redo.size()), pr(redo.size());
-			for (size_t i = 0; i < redo.size(); ++i) { pq[i] = redo[i] / n_r; pr[i] = redo[i] % n_r; }
+			for (size_t i = 0; i < redo.size(); ++i) { pq[i] = (int32_t)(redo[i] / n_r); pr[i] = (int32_t)(redo[i] % n_r); }
 			std::vector<ssw_batch_result> sub(redo.size());
 			const ssw_engine_timing keep_t = e->timing;
 			rc = align_general(e, P0, S, (int64_t)redo.size(), pq.data(), pr.data(), sub.data(), nullptr, 0, &no_pool);

@@ -262,6 +262,55 @@ ssw_grid_select_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGrid
 	if (tid == 0) n_hits[q] = cnt;
 }
 
+/* Top-k search over grid tiles: one CTA per query slot (pi, half) of a launch group of a later tile, run after the selection
+ * kernel wrote the slot's row to the tile table (t_*; reference numbers of the tile, offset by r_base here).  Row q of the
+ * running table becomes the first min(k, n_a + n_b) of the two rows in rank order -- in place: every thread reads its entries
+ * before the barrier and writes them after it.  Every reference of the tile has a larger number than every reference of the
+ * running row, so the keys are distinct and the result is the selection over the union (grid hits never have status 1).
+ * Output i comes from the merge path: x entries of the running row and i - x of the tile row precede it. */
+__global__ void __launch_bounds__(SSW_SELECT_THREADS)
+ssw_grid_merge_kernel(const int2* __restrict__ qp, int32_t k, int32_t r_base,
+                      int32_t* __restrict__ hit_ref, ssw_batch_result* __restrict__ hits, int32_t* __restrict__ n_hits,
+                      const int32_t* __restrict__ t_ref, const ssw_batch_result* __restrict__ t_hits, const int32_t* __restrict__ t_n)
+{
+	constexpr int kPer = SSW_SEARCH_MAX_K / SSW_SELECT_THREADS;      /* outputs per thread */
+	__shared__ uint64_t s_a[SSW_SEARCH_MAX_K], s_b[SSW_SEARCH_MAX_K];
+	const int h = (int)(blockIdx.x & 1), pi = (int)(blockIdx.x >> 1);
+	const int2 pr = qp[pi];
+	const int q = h ? pr.y : pr.x;
+	if (q < 0) return;                                 /* the whole CTA: no second query in this pair-task */
+	const int tid = threadIdx.x;
+	const int64_t row = (int64_t)q * k;
+	const int na = n_hits[q], nb = t_n[q];
+	for (int i = tid; i < na; i += SSW_SELECT_THREADS) s_a[i] = ssw_hit_key(hits[row + i].score1, hit_ref[row + i]);
+	for (int i = tid; i < nb; i += SSW_SELECT_THREADS) s_b[i] = ssw_hit_key(t_hits[row + i].score1, r_base + t_ref[row + i]);
+	__syncthreads();
+	const int cnt = min(k, na + nb);
+	ssw_batch_result o[kPer];
+	int32_t ref[kPer];
+#pragma unroll
+	for (int j = 0; j < kPer; ++j) {
+		const int i = tid + j * SSW_SELECT_THREADS;
+		if (i < cnt) {
+			int lo = max(0, i - nb), hi = min(i, na);
+			while (lo < hi) {
+				const int m = (lo + hi) >> 1;
+				if (s_a[m] < s_b[i - 1 - m]) lo = m + 1; else hi = m;
+			}
+			const int y = i - lo;
+			if (y >= nb || (lo < na && s_a[lo] < s_b[y])) { o[j] = hits[row + lo]; ref[j] = hit_ref[row + lo]; }
+			else { o[j] = t_hits[row + y]; ref[j] = r_base + t_ref[row + y]; }
+		}
+	}
+	__syncthreads();
+#pragma unroll
+	for (int j = 0; j < kPer; ++j) {
+		const int i = tid + j * SSW_SELECT_THREADS;
+		if (i < cnt) { hits[row + i] = o[j]; hit_ref[row + i] = ref[j]; }
+	}
+	if (tid == 0) n_hits[q] = cnt;
+}
+
 /* ---- threshold search (ssw_engine_search_all): every hit, compacted in reference order ----------------------------------- */
 
 /* One CTA per query slot (pi, half) of a launch group, as the selection kernel: slot_n[slot] receives the number of hits of

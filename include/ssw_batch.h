@@ -120,6 +120,9 @@ int ssw_engine_align(ssw_engine* e, const ssw_batch_params* params,
  *              (ssw_engine_timing.leftover_pairs counts them).  One long reference costs its own column of the grid, not
  *              the device path.  Conditions on the call -- gap_open <= gap_extend, the "chunk" option -- still send every
  *              pair down the general path.
+ *   size       a grid of more than 2^31 - 1 pairs, or one whose references need more scratch per query pair than a launch
+ *              may take, is cut into grid tiles (contiguous runs of references), each run on the device; the k best of
+ *              every tile are merged into each query's k best on the device, and the hit table still comes back in one copy.
  */
 int ssw_engine_search(ssw_engine* e, const ssw_batch_params* params, int32_t k, int32_t min_score,
                       int32_t* hit_ref, ssw_batch_result* hits, int32_t* n_hits,
@@ -139,7 +142,8 @@ int ssw_engine_search(ssw_engine* e, const ssw_batch_params* params, int32_t k, 
  *              hits only, into a CIGAR pool the set owns (cigar_off counts words of that pool, at most 2^31 of them)
  *   max_hits   >= 0; a call that finds more hits returns -2 and no set (it may stop as soon as its running count passes the
  *              bound: the guard against a low min_score on a grid of 10^8 pairs)
- * The result does not depend on the path that ran, on how the grid was cut into launch groups or on the number of devices.
+ * The result does not depend on the path that ran, on how the grid was cut into launch groups or grid tiles (as for
+ * ssw_engine_search) or on the number of devices.
  * Where the grid path runs, the hits of every launch group are counted and compacted on the device and copied back while the
  * next group computes: no record of a non-hit crosses to the host, and the device holds one launch group's hits at a time.
  * Which pairs run where is as for ssw_engine_search.  Every failure leaves *out NULL.
@@ -319,6 +323,9 @@ int ssw_engine_set_option(ssw_engine* e, const char* name, int64_t value);
  *   "grid_order"    1 (default): the items of a query pair sweep the references longest first, so that the groups of a warp,
  *                   which run as long as their longest item, end together; 0: in reference order (measurements)
  *   "grid_max_ref"  references longer than this are not planned on the device (default and largest value 65,536; tests)
+ *   "grid_tile_refs" ssw_engine_search / ssw_engine_search_all: at most this many qualifying references per grid tile (0,
+ *                   the default: automatic -- one tile unless the grid has more than 2^31 - 1 pairs or one query pair's scratch
+ *                   over all references exceeds the launch budget; tests, measurements).  Changes no result.
  */
 
 #ifdef __cplusplus
