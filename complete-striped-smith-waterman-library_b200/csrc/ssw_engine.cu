@@ -20,6 +20,7 @@
 #include <string.h>
 #include <math.h>
 #include <functional>
+#include <map>
 #include <utility>
 
 #include "ssw_common.cuh"
@@ -108,7 +109,8 @@ struct SswOptions {
 	int force_inst = -1;            /* "inst" (measurements): use this forward instance whenever it covers the query */
 	int tb_maxbw = SSW_TBP_MAXBW;   /* "tb_maxbw": widest band handled by the shared-memory traceback kernel */
 	int tb_spec = -1;               /* "tb_spec": 1 = band-doubling rounds of a task side by side (speculative kernel), 0 = one after the other, -1 = automatic (small batches) */
-	int cm_block = -1;              /* "cm_block": -1 automatic, 0 one word per column always, 1 block maxima wherever chunking is possible (tests) */
+	int cm_block = -1;              /* "cm_block": -1 automatic, 0 one word per column always, 1 exact block maxima wherever chunking is
+	                                 * possible (tests), 2 bounded block words (CM == 3) wherever chunking is possible (tests) */
 	int64_t chunk = 0;              /* "chunk": reference chunk length of the fill kernel (0 automatic) */
 	int64_t small_chunk = 0;        /* "small_chunk" (measurements): chunk length of launches too small to fill the device */
 	int64_t cm_budget = 0;          /* "cm_budget_mb": cap of the column-maximum scratch per launch in bytes (0: half of the free memory; tests) */
@@ -124,7 +126,7 @@ static const SswOptionDef kOptions[] = {
 	{"parts", [](SswOptions& o, int64_t v) { o.strip_parts = v == 1 || v == 2 || v == 4 ? (int)v : 0; }},
 	{"small_chunk", [](SswOptions& o, int64_t v) { o.small_chunk = v < 0 ? 0 : (v + 3) / 4 * 4; }},
 	{"chunk", [](SswOptions& o, int64_t v) { o.chunk = v < 0 ? 0 : (v + 3) / 4 * 4; }},
-	{"cm_block", [](SswOptions& o, int64_t v) { o.cm_block = v < 0 ? -1 : (v ? 1 : 0); }},
+	{"cm_block", [](SswOptions& o, int64_t v) { o.cm_block = v < 0 ? -1 : (int)std::min<int64_t>(v, 2); }},
 	{"cm_budget_mb", [](SswOptions& o, int64_t v) { o.cm_budget = v <= 0 ? 0 : v << 20; }},
 	{"grid_split", [](SswOptions& o, int64_t v) { o.grid_split_pairs = v < 0 ? (int64_t)4 << 20 : v; }},
 	{"grid_arm", [](SswOptions& o, int64_t v) { o.grid_arm = v < 0 ? -1 : (int)v; }},
@@ -189,6 +191,7 @@ struct ssw_engine {
 	SswDevBuf d_hits;                                        /* ssw_engine_search: the n_q x k hit table of the grid path */
 	SswDevBuf d_mark;                                        /* ssw_engine_mark_mismatch: tasks, input CIGARs, marked CIGARs */
 	SswDevBuf d_rf_items, d_rf_bests, d_rf_blk, d_rf_cm;     /* block-maximum mode: re-fill items, their (unused) bests, first columns, column maxima */
+	SswDevBuf d_bd_items, d_bd_bests, d_bd_cm, d_bd_cand, d_bd_cnt;   /* bounded block words: candidate re-fills, candidate lists, counts + offsets */
 	int64_t last_cm_words = 0;                               /* column-maximum words of the last forward launch (ssw_engine_last_colmax) */
 	SswStagedD2H staged;
 	cudaStream_t side[3] = {nullptr, nullptr, nullptr};     /* traceback launches of different kernel shapes run side by side */
@@ -250,7 +253,7 @@ static int fill_items_per_cta(int inst, int n)
 template <int G, int R>
 static int launch_fill(ssw_engine* e, const FillPtrs& fp, int n_items, int dir, int cm_mode, int share, const ssw_batch_params& P)
 {
-	const FillShape sh = fill_shape<R>(P.n, share, dir, !(dir > 0 && cm_mode == 2));
+	const FillShape sh = fill_shape<R>(P.n, share, dir, !(dir > 0 && cm_mode >= 2));
 	if (sh.smem > 220 * 1024) { fprintf(stderr, "[libssw-b200] alphabet of %d letters is too large for this query length\n", P.n); return -2; }
 	const int per_cta = sh.warps * (32 / G);
 	const int grid = (n_items + per_cta - 1) / per_cta;
@@ -272,11 +275,13 @@ static int launch_fill(ssw_engine* e, const FillPtrs& fp, int n_items, int dir, 
 	if (sh.warps == 8) {
 		if constexpr (R >= 16) {
 			if (cm_mode == 2) return go(ssw_fill_kernel<G, R, 1, 2, false, 8, false>);
+			if (cm_mode == 3) return go(ssw_fill_kernel<G, R, 1, 3, false, 8, false>);
 			return fp.arm ? go(ssw_fill_kernel<G, R, 1, 1, false, 8, true>) : go(ssw_fill_kernel<G, R, 1, 1, false, 8, false>);
 		}
 		return -2;
 	}
 	if (cm_mode == 2) return go(ssw_fill_kernel<G, R, 1, 2, false, SSW_FILL_WARPS, false>);
+	if (cm_mode == 3) return go(ssw_fill_kernel<G, R, 1, 3, false, SSW_FILL_WARPS, false>);
 	return fp.arm ? go(ssw_fill_kernel<G, R, 1, 1, false, SSW_FILL_WARPS, true>) : go(ssw_fill_kernel<G, R, 1, 1, false, SSW_FILL_WARPS, false>);
 }
 
@@ -357,7 +362,8 @@ extern "C" void ssw_engine_destroy(ssw_engine* e)
 {
 	if (!e) return;
 	cudaSetDevice(e->device);
-	SswDevBuf* bufs[] = {&e->d_q, &e->d_r, &e->d_mat, &e->d_items, &e->d_bests, &e->d_alns, &e->d_res, &e->d_colmax, &e->d_tb, &e->d_bnd, &e->d_park, &e->d_emul, &e->d_grid, &e->d_out, &e->d_sync, &e->d_rf_items, &e->d_rf_bests, &e->d_rf_blk, &e->d_rf_cm, &e->d_mark, &e->d_hits};
+	SswDevBuf* bufs[] = {&e->d_q, &e->d_r, &e->d_mat, &e->d_items, &e->d_bests, &e->d_alns, &e->d_res, &e->d_colmax, &e->d_tb, &e->d_bnd, &e->d_park, &e->d_emul, &e->d_grid, &e->d_out, &e->d_sync, &e->d_rf_items, &e->d_rf_bests, &e->d_rf_blk, &e->d_rf_cm, &e->d_mark, &e->d_hits,
+	                     &e->d_bd_items, &e->d_bd_bests, &e->d_bd_cm, &e->d_bd_cand, &e->d_bd_cnt};
 	for (SswDevBuf* b : bufs) b->release();
 	for (ssw_engine*& k : e->kids) if (k) { ssw_engine_destroy(k); k = nullptr; }
 	e->staged.release();
@@ -670,7 +676,28 @@ static inline bool needs_other(const SswFillResult& r, int word, const Sem& S, b
 /* How the column maxima of the fill being resolved are stored (fill kernel CM mode), and -- block mode -- what the
  * re-fill of single blocks needs: a kernel instance that covers the rows of every alignment (those of the fill, or the
  * byte padding of alignments filled on their word rows: rows >= an item's lp are dead) and the scoring parameters. */
-struct CmMode { int block; int inst; const ssw_batch_params* P; };
+/* block: 0 one word per column, 1 exact block maxima (CM == 2), 2 bounded block words (CM == 3).  fill_inst: the instance of the
+ * fill (bounded words: the pair-task of an alignment over the candidate cap re-runs with it).  colmax / items: the words and the
+ * fill items the descriptors point into (nullptr: the engine's d_colmax / d_items). */
+struct CmMode { int block; int inst; const ssw_batch_params* P; int fill_inst = -1; const uint32_t* colmax = nullptr; const SswItem* items = nullptr; };
+
+/* Host side of a candidate stage of the bounded block words: read the per-alignment counts (-1: over the cap), turn them into
+ * offsets on the device and mark the alignments over the cap.  Returns the number of candidates, -1 on an error. */
+static int64_t bound_offsets(ssw_engine* e, size_t n_aln, const int32_t* d_cnt, int32_t* d_off, std::vector<char>& exact)
+{
+	std::vector<int32_t> cnt(n_aln), off(n_aln);
+	if (cudaMemcpyAsync(cnt.data(), d_cnt, sizeof(int32_t) * n_aln, cudaMemcpyDeviceToHost, e->stream) != cudaSuccess ||
+	    cudaStreamSynchronize(e->stream) != cudaSuccess) return -1;
+	int64_t total = 0;
+	for (size_t i = 0; i < n_aln; ++i) {
+		off[i] = (int32_t)total;
+		if (cnt[i] < 0) exact[i] = 1; else total += cnt[i];
+	}
+	if (total > INT32_MAX / SSW_CM_BLOCK) { fprintf(stderr, "[libssw-b200] too many candidate blocks in one resolve (%lld)\n", (long long)total); return -1; }
+	if (cudaMemcpyAsync(d_off, off.data(), sizeof(int32_t) * n_aln, cudaMemcpyHostToDevice, e->stream) != cudaSuccess ||
+	    cudaStreamSynchronize(e->stream) != cudaSuccess) return -1;     /* `off` is a local: wait for the copy */
+	return total;
+}
 
 /* Launch the resolve kernel(s) over `descs` and fetch the results. */
 static int run_resolve(ssw_engine* e, const std::vector<SswAlnDesc>& descs, bool second, std::vector<SswFillResult>& res, const CmMode* cm = nullptr)
@@ -683,33 +710,84 @@ static int run_resolve(ssw_engine* e, const std::vector<SswAlnDesc>& descs, bool
 	e->laps.start(e->stream);
 	const int per = SSW_RESOLVE_THREADS / 32;
 	const dim3 grid(((int)descs.size() + per - 1) / per);
+	std::vector<char> exact;        /* bounded words: alignments over the candidate cap */
 	if (cm && cm->block) {
-		/* block maxima (the fill kept no item bests, so this runs whether or not the second best is wanted): stage 0 (the first
-		 * block holding the score) and its re-fill with best-cell tracking, stage 1 (the best cell + the three blocks per
-		 * alignment that need single columns, and the columns right of the mask window of byte alignments filled on their word
-		 * rows), re-fill of those ranges with one word per column, stage 2.  Scratch: SSW_REFILL_SLOTS items per alignment,
-		 * then one best-block item per alignment. */
+		const uint32_t* colmax = cm->colmax ? cm->colmax : e->d_colmax.as<uint32_t>();
+		const SswItem* items = cm->items ? cm->items : e->d_items.as<SswItem>();
+		const SswAlnDesc* alns = e->d_alns.as<SswAlnDesc>();
+		/* block words (the fill kept no item bests, so this runs whether or not the second best is wanted).  Exact maxima: stage 0
+		 * (the first block holding the score) and its re-fill with best-cell tracking; bounded words: the C1 candidates and their
+		 * re-fills with tracking.  Then stage 1 (the best cell + the blocks cut by the mask window, and the columns right of it of
+		 * byte alignments filled on their word rows; exact maxima: the first block of the largest fully allowed block maximum,
+		 * bounded words: the C2 candidates), re-fill of those ranges with one word per column, stage 2.  Scratch:
+		 * SSW_REFILL_SLOTS items per alignment, then (exact maxima) one best-block item per alignment. */
 		const size_t n_aln = descs.size(), n_rf = n_aln * SSW_REFILL_SLOTS;
 		if (e->d_rf_items.ensure(sizeof(SswItem) * (n_rf + n_aln))) return -1;
 		if (e->d_rf_bests.ensure(sizeof(SswItemBest) * (n_rf + n_aln))) return -1;
 		if (e->d_rf_blk.ensure(sizeof(int32_t) * n_rf)) return -1;    /* first column of every re-filled range, -1: none */
 		if (e->d_rf_cm.ensure(sizeof(uint32_t) * n_rf * SSW_CM_BLOCK + 64)) return -1;
-		ssw_launch(ssw_resolve_best_block_kernel<0>, grid, dim3(SSW_RESOLVE_THREADS), 0, e->stream, (const SswAlnDesc*)e->d_alns.as<SswAlnDesc>(),
-		           (int)n_aln, (const uint32_t*)e->d_colmax.as<uint32_t>(), (const SswItem*)e->d_items.as<SswItem>(), e->d_rf_items.as<SswItem>() + n_rf);
-		SSW_CUDA_OK(cudaGetLastError());
-		const FillPtrs fp_best = {e->d_rf_items.as<SswItem>() + n_rf, e->d_rf_cm.as<uint32_t>(), e->d_rf_bests.as<SswItemBest>() + n_rf};
-		int rc = dispatch_fill(e, cm->inst, fp_best, (int)n_aln, +1, 1, 0, *cm->P);
-		if (rc) return rc < 0 ? rc : -1;
-		ssw_launch(ssw_resolve_blocks_kernel<0>, grid, dim3(SSW_RESOLVE_THREADS), 0, e->stream, (const SswAlnDesc*)e->d_alns.as<SswAlnDesc>(),
-		           (int)n_aln, (const SswItemBest*)e->d_rf_bests.as<SswItemBest>() + n_rf, (const uint32_t*)e->d_colmax.as<uint32_t>(),
-		           (const SswItem*)e->d_items.as<SswItem>(), e->d_res.as<SswFillResult>(), e->d_rf_items.as<SswItem>(), e->d_rf_blk.as<int32_t>());
-		SSW_CUDA_OK(cudaGetLastError());
 		const FillPtrs fp = {e->d_rf_items.as<SswItem>(), e->d_rf_cm.as<uint32_t>(), e->d_rf_bests.as<SswItemBest>()};
-		rc = dispatch_fill(e, cm->inst, fp, (int)n_rf, +1, 1, 0, *cm->P);
-		if (rc) return rc < 0 ? rc : -1;
-		ssw_launch(ssw_resolve_refill_kernel<0>, grid, dim3(SSW_RESOLVE_THREADS), 0, e->stream, (const SswAlnDesc*)e->d_alns.as<SswAlnDesc>(),
-		           (int)n_aln, (const int32_t*)e->d_rf_blk.as<int32_t>(), (const uint32_t*)e->d_rf_cm.as<uint32_t>(), e->d_res.as<SswFillResult>());
-		e->timing.other_launches += 4;
+		if (cm->block == 1) {
+			ssw_launch(ssw_resolve_best_block_kernel<0>, grid, dim3(SSW_RESOLVE_THREADS), 0, e->stream, alns, (int)n_aln, colmax, items,
+			           e->d_rf_items.as<SswItem>() + n_rf);
+			SSW_CUDA_OK(cudaGetLastError());
+			const FillPtrs fp_best = {e->d_rf_items.as<SswItem>() + n_rf, e->d_rf_cm.as<uint32_t>(), e->d_rf_bests.as<SswItemBest>() + n_rf};
+			int rc = dispatch_fill(e, cm->inst, fp_best, (int)n_aln, +1, 1, 0, *cm->P);
+			if (rc) return rc < 0 ? rc : -1;
+			ssw_launch(ssw_resolve_blocks_kernel<false>, grid, dim3(SSW_RESOLVE_THREADS), 0, e->stream, alns, (int)n_aln,
+			           (const SswItemBest*)e->d_rf_bests.as<SswItemBest>() + n_rf, colmax, items, e->d_res.as<SswFillResult>(),
+			           e->d_rf_items.as<SswItem>(), e->d_rf_blk.as<int32_t>(), (const int32_t*)nullptr, (const int32_t*)nullptr,
+			           SswBound{0, 0, 0}, (int32_t*)nullptr, (int32_t*)nullptr);
+			SSW_CUDA_OK(cudaGetLastError());
+			rc = dispatch_fill(e, cm->inst, fp, (int)n_rf, +1, 1, 0, *cm->P);
+			if (rc) return rc < 0 ? rc : -1;
+			ssw_launch(ssw_resolve_refill_kernel<0>, grid, dim3(SSW_RESOLVE_THREADS), 0, e->stream, alns, (int)n_aln,
+			           (const int32_t*)e->d_rf_blk.as<int32_t>(), (const uint32_t*)e->d_rf_cm.as<uint32_t>(), e->d_res.as<SswFillResult>(),
+			           (const int32_t*)nullptr, 0, (const int32_t*)nullptr, (const int32_t*)nullptr, (const uint32_t*)nullptr);
+			e->timing.other_launches += 4;
+		} else {
+			const SswBound bd = {(int)cm->P->gap_open, (int)cm->P->gap_extend, SSW_BOUND_CAP};
+			if (e->d_bd_cand.ensure(sizeof(int32_t) * n_aln * (size_t)bd.cap + 64)) return -1;
+			if (e->d_bd_cnt.ensure(sizeof(int32_t) * 4 * n_aln)) return -1;
+			int32_t* cnt1 = e->d_bd_cnt.as<int32_t>();
+			int32_t* cnt2 = cnt1 + n_aln, *off1 = cnt2 + n_aln, *off2 = off1 + n_aln;
+			int32_t* cand = e->d_bd_cand.as<int32_t>();
+			exact.assign(n_aln, 0);
+			ssw_launch(ssw_bound_best_kernel<0>, grid, dim3(SSW_RESOLVE_THREADS), 0, e->stream, alns, (int)n_aln, colmax, bd, cand, cnt1);
+			SSW_CUDA_OK(cudaGetLastError());
+			const int64_t n1 = bound_offsets(e, n_aln, cnt1, off1, exact);
+			if (n1 < 0) return -1;
+			if (e->d_bd_items.ensure(sizeof(SswItem) * (size_t)n1 + 64)) return -1;
+			if (e->d_bd_bests.ensure(sizeof(SswItemBest) * (size_t)n1 + 64)) return -1;
+			ssw_launch(ssw_bound_emit_kernel<0>, grid, dim3(SSW_RESOLVE_THREADS), 0, e->stream, alns, (int)n_aln, items, (const int32_t*)cand,
+			           bd.cap, (const int32_t*)cnt1, (const int32_t*)off1, 0, e->d_bd_items.as<SswItem>());
+			SSW_CUDA_OK(cudaGetLastError());
+			const FillPtrs fp1 = {e->d_bd_items.as<SswItem>(), e->d_rf_cm.as<uint32_t>(), e->d_bd_bests.as<SswItemBest>()};
+			int rc = n1 > 0 ? dispatch_fill(e, cm->inst, fp1, (int)n1, +1, 1, 0, *cm->P) : 0;
+			if (rc) return rc < 0 ? rc : -1;
+			ssw_launch(ssw_resolve_blocks_kernel<true>, grid, dim3(SSW_RESOLVE_THREADS), 0, e->stream, alns, (int)n_aln,
+			           (const SswItemBest*)e->d_bd_bests.as<SswItemBest>(), colmax, items, e->d_res.as<SswFillResult>(),
+			           e->d_rf_items.as<SswItem>(), e->d_rf_blk.as<int32_t>(), (const int32_t*)cnt1, (const int32_t*)off1, bd, cand, cnt2);
+			SSW_CUDA_OK(cudaGetLastError());
+			const int64_t n2 = bound_offsets(e, n_aln, cnt2, off2, exact);
+			if (n2 < 0) return -1;
+			if (e->d_bd_items.ensure(sizeof(SswItem) * (size_t)n2 + 64)) return -1;
+			if (e->d_bd_bests.ensure(sizeof(SswItemBest) * (size_t)n2 + 64)) return -1;
+			if (e->d_bd_cm.ensure(sizeof(uint32_t) * (size_t)n2 * SSW_CM_BLOCK + 64)) return -1;
+			ssw_launch(ssw_bound_emit_kernel<0>, grid, dim3(SSW_RESOLVE_THREADS), 0, e->stream, alns, (int)n_aln, items, (const int32_t*)cand,
+			           bd.cap, (const int32_t*)cnt2, (const int32_t*)off2, 1, e->d_bd_items.as<SswItem>());
+			SSW_CUDA_OK(cudaGetLastError());
+			rc = dispatch_fill(e, cm->inst, fp, (int)n_rf, +1, 1, 0, *cm->P);
+			if (rc) return rc < 0 ? rc : -1;
+			const FillPtrs fp2 = {e->d_bd_items.as<SswItem>(), e->d_bd_cm.as<uint32_t>(), e->d_bd_bests.as<SswItemBest>()};
+			rc = n2 > 0 ? dispatch_fill(e, cm->inst, fp2, (int)n2, +1, 1, 0, *cm->P) : 0;
+			if (rc) return rc < 0 ? rc : -1;
+			ssw_launch(ssw_resolve_refill_kernel<0>, grid, dim3(SSW_RESOLVE_THREADS), 0, e->stream, alns, (int)n_aln,
+			           (const int32_t*)e->d_rf_blk.as<int32_t>(), (const uint32_t*)e->d_rf_cm.as<uint32_t>(), e->d_res.as<SswFillResult>(),
+			           (const int32_t*)cand, bd.cap, (const int32_t*)cnt2, (const int32_t*)off2, (const uint32_t*)e->d_bd_cm.as<uint32_t>());
+			e->timing.other_launches += 6 + (n1 > 0 ? 1 : 0) + (n2 > 0 ? 1 : 0);
+			e->timing.block_refills += n1 + n2;
+		}
 	} else if (second)
 		ssw_launch(ssw_resolve_kernel<true>, grid, dim3(SSW_RESOLVE_THREADS), 0, e->stream, (const SswAlnDesc*)e->d_alns.as<SswAlnDesc>(),
 		           (int)descs.size(), (const SswItemBest*)e->d_bests.as<SswItemBest>(), (const uint32_t*)e->d_colmax.as<uint32_t>(), e->d_res.as<SswFillResult>());
@@ -721,6 +799,47 @@ static int run_resolve(ssw_engine* e, const std::vector<SswAlnDesc>& descs, bool
 	e->timing.other_launches += 1;
 	SSW_CUDA_OK(cudaMemcpyAsync(res.data(), e->d_res.p, sizeof(SswFillResult) * descs.size(), cudaMemcpyDeviceToHost, e->stream));
 	SSW_CUDA_OK(cudaStreamSynchronize(e->stream));
+	if (std::find(exact.begin(), exact.end(), 1) == exact.end()) return 0;
+
+	/* Alignments over the candidate cap: their pair-tasks re-run with exact block maxima into rows of a scratch of their own (the
+	 * bounded words stay as they are, for a second resolve of the same fill), and the alignments are resolved from those. */
+	std::vector<int64_t> fb;
+	for (size_t i = 0; i < exact.size(); ++i) if (exact[i]) fb.push_back((int64_t)i);
+	std::vector<SswItem> fb_items;
+	std::vector<SswAlnDesc> fb_descs;
+	std::map<int32_t, int32_t> task;            /* first item of a pair-task -> its first item in the scratch */
+	int64_t words = 0;
+	const SswItem* items = cm->items ? cm->items : e->d_items.as<SswItem>();
+	for (int64_t i : fb) {
+		SswAlnDesc d = descs[(size_t)i];
+		auto it = task.find(d.first_item);
+		if (it == task.end()) {
+			const size_t at = fb_items.size();
+			fb_items.resize(at + (size_t)d.n_items);
+			SSW_CUDA_OK(cudaMemcpy(fb_items.data() + at, items + d.first_item, sizeof(SswItem) * (size_t)d.n_items, cudaMemcpyDeviceToHost));
+			for (size_t k = at; k < fb_items.size(); ++k) fb_items[k].cm_off = words;
+			words += ((int64_t)d.ref_len / SSW_CM_BLOCK + 1 + 3) / 4 * 4;
+			it = task.emplace(d.first_item, (int32_t)at).first;
+		}
+		d.cm_off = fb_items[(size_t)it->second].cm_off;
+		d.first_item = it->second;
+		fb_descs.push_back(d);
+	}
+	if (e->d_bd_items.ensure(sizeof(SswItem) * fb_items.size())) return -1;
+	if (e->d_bd_cm.ensure(sizeof(uint32_t) * (size_t)words + 64)) return -1;
+	SSW_CUDA_OK(cudaMemcpyAsync(e->d_bd_items.p, fb_items.data(), sizeof(SswItem) * fb_items.size(), cudaMemcpyHostToDevice, e->stream));
+	e->laps.start(e->stream);
+	const FillPtrs fpx = {e->d_bd_items.as<SswItem>(), e->d_bd_cm.as<uint32_t>(), e->d_rf_bests.as<SswItemBest>()};
+	const int rc = dispatch_fill(e, cm->fill_inst, fpx, (int)fb_items.size(), +1, 2, 0, *cm->P);
+	if (rc) return rc < 0 ? rc : -1;
+	e->laps.stop(e->stream, &e->timing.resolve_ms);
+	e->timing.other_launches += 1;
+	e->timing.block_exact += (int64_t)fb.size();
+	CmMode cx = *cm;
+	cx.block = 1; cx.colmax = e->d_bd_cm.as<uint32_t>(); cx.items = e->d_bd_items.as<SswItem>();
+	std::vector<SswFillResult> fb_res;
+	if (run_resolve(e, fb_descs, second, fb_res, &cx)) return -1;
+	for (size_t j = 0; j < fb.size(); ++j) res[(size_t)fb[j]] = fb_res[j];
 	return 0;
 }
 
@@ -1066,7 +1185,10 @@ static int forward_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Al
 		/* Column maxima: one word per column, or -- long references in a launch that fills the device -- one word per block of
 		 * SSW_CM_BLOCK columns plus a re-fill of the three blocks per alignment whose single columns matter (ssw_resolve.cuh).
 		 * The re-fill needs a bounded warm-up, i.e. the same condition as chunking. */
+		/* Block words: exact block maxima ("cm_block" 1) or, by default, the bounded words of CM == 3 (DESIGN 2), which need
+		 * gapE > 0 as chunking does. */
 		bool block = e->opt.cm_block != 0 && P.gap_extend > 0 && S.max_mat > 0;
+		const bool bounded = e->opt.cm_block != 1;
 		if (block && e->opt.cm_block < 0) {
 			if (latency) block = false;
 			for (size_t i = k; block && i < pts.size() && pts[i].inst == inst; ++i) if (e->r_len[pts[i].r] < 32768) block = false;
@@ -1202,13 +1324,13 @@ static int forward_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Al
 		}
 		tr.lap("forward: plan");
 		if (e->d_colmax.ensure(cm_words * 4 + 64)) return -1;
-		if (e->run_fill(items, inst, +1, block ? 2 : 1, share, P, &e->timing.fill_forward_ms)) return -1;
+		if (e->run_fill(items, inst, +1, block ? (bounded ? 3 : 2) : 1, share, P, &e->timing.fill_forward_ms)) return -1;
 		e->last_cm_words = (int64_t)cm_words;
 		tr.lap("forward: fill (copy+kernel)");
 		e->timing.fill_forward_launches += 1;
 		e->timing.cells_forward += cells;
 		const int rows = inst_rows(inst);
-		const CmMode cm_mode = {block ? 1 : 0, rf_lp > rows ? pick_inst(rf_lp, -1) : inst, &P};
+		const CmMode cm_mode = {block ? (bounded ? 2 : 1) : 0, rf_lp > rows ? pick_inst(rf_lp, -1) : inst, &P, inst};
 		/* The word results of byte overflows filled on their word rows are resolved from this launch when it holds every
 		 * pair-task of its kernel instance (the BASELINE shapes: config 3 is one launch per GPU, which then needs no second
 		 * one).  Where the column-maximum budget cuts an instance into several launches, those overflows keep the word
@@ -2043,6 +2165,7 @@ static int engine_align_impl(ssw_engine* e, const ssw_batch_params* params,
 				e->timing.fill_reverse_ms += t.fill_reverse_ms; e->timing.traceback_ms += t.traceback_ms;
 				e->timing.fill_forward_launches += t.fill_forward_launches; e->timing.other_launches += t.other_launches;
 				e->timing.cells_forward += t.cells_forward; e->timing.byte_overflows += t.byte_overflows;
+				e->timing.block_refills += t.block_refills; e->timing.block_exact += t.block_exact;
 			}
 			e->timing.total_ms = e->t_total.stop(e->stream);
 			e->laps.collect();

@@ -30,7 +30,7 @@
  *                           from a boundary buffer a few columns behind its producer.
  *
  * Outputs per item: the lexicographic best cell (score, first scan position,
- * smallest row) per half -- not in block mode (CM == 2) -- and, forward pass,
+ * smallest row) per half -- not in block mode (CM == 2, 3) -- and, forward pass,
  * the column maxima over real and pad rows (the reference's maxColumn[],
  * ssw.c:338/:540) as packed s16x2 words.  All order-dependent semantics (strict
  * '>' running maximum, byte overflow, mask window) are applied afterwards by
@@ -370,7 +370,10 @@ __device__ static __forceinline__ void ssw_reduce_best(const SswLaneBest& lb, in
  *      single columns only in the first block holding the largest block maximum, the second-best scan (ssw.c:368-381) only
  *      in the <= 2 blocks cut by the mask window and in the block that holds the winner; ssw_resolve.cuh re-fills those
  *      blocks per alignment with mode 1.  Chunks start at multiples of SSW_CM_BLOCK, and so does every item's sweep
- *      (p0 - warm: the planner rounds the warm-up up to a multiple of SSW_CM_BLOCK). */
+ *      (p0 - warm: the planner rounds the warm-up up to a multiple of SSW_CM_BLOCK).
+ *   3  as 2, but the word of a block is w(b), the largest row maximum of E sampled once per loop body over the block, which
+ *      brackets the block maximum M(b): w + gapE <= M <= w + gapO + 7 gapE (DESIGN 2; the lower bound of a body that straddles
+ *      a block boundary belongs to the later block).  ssw_resolve.cuh re-fills only the blocks the bracket cannot rule out. */
 /* WARPS: warps per CTA.  4 by default; 8 where one CTA-shared profile is so large (protein alphabets: 64 KB at 20 rows per
  * lane) that four-warp CTAs would leave the SM with 8 resident warps -- eight warps per profile keep 16. */
 /* ARM: items may carry a late arming position (SswItem.cend, device-planned grids); a template parameter so that the kernels
@@ -419,11 +422,12 @@ ssw_fill_kernel(const SswItem* __restrict__ items, int n_items,
 	/* ---- sweep ---- */
 	const uint8_t* rp = reinterpret_cast<const uint8_t*>(refs) + it.ref_off;   /* reference column 0 */
 	const uint32_t negO = pack2(-gapO, -gapO), negE = pack2(-gapE, -gapE);
-	int sL = (it.p0 - it.warm - (G - 1)) & (CM == 2 ? ~7 : ~3);   /* scan position of the group's last lane, multiple of 4 (block mode: of 8) */
+	constexpr bool BLK = CM == 2 || CM == 3;            /* block mode: one word per SSW_CM_BLOCK columns */
+	int sL = (it.p0 - it.warm - (G - 1)) & (BLK ? ~7 : ~3);   /* scan position of the group's last lane, multiple of 4 (block mode: of 8) */
 	constexpr int U = 8;                                /* scan positions per loop body */
 	/* block mode sweeps on to the end of the last block, so that its last lane finishes that block inside the loop (the
 	 * columns behind the reference leave the block maximum as it is, see the block fold below) */
-	const int p_end = CM == 2 ? (it.p1 + SSW_CM_BLOCK - 1) & ~(SSW_CM_BLOCK - 1) : it.p1;
+	const int p_end = BLK ? (it.p1 + SSW_CM_BLOCK - 1) & ~(SSW_CM_BLOCK - 1) : it.p1;
 	int n_body = live && it.p1 > sL ? (p_end - sL + U - 1) / U : 0;
 	/* the longest group's count, in a uniform register (REDUX): the loop branch is then uniform, and ptxas issues the
 	 * shuffles of the step without the per-step WARPSYNC.COLLECTIVE guards and register copies of a loop it cannot
@@ -456,19 +460,21 @@ ssw_fill_kernel(const SswItem* __restrict__ items, int n_items,
 	uint32_t outH = 0, outF = 0, outC = 0;
 	/* Block mode keeps no best cell: the resolve takes the score and the first block holding it from the block maxima and
 	 * re-fills that one block with tracking (ssw_resolve.cuh).  So its sweep carries only the recurrence and the maxima. */
-	constexpr bool TRACK = CM != 2;
+	constexpr bool TRACK = !BLK;
 	/* Block mode computes the cells in the form with 3 ALU-pipe instructions per cell pair (ssw_cells); the other instances
 	 * keep the 4-instruction form, since the 3-instruction form has been timed only in block mode (configs 2 and 3). */
-	constexpr bool FROM_H = CM == 2;
+	constexpr bool FROM_H = BLK;
 	SswLaneBest lb;
 	lb.best = 0; lb.pos0 = lb.pos1 = -1; lb.row0 = lb.row1 = 0;      /* position -1: no recorded event (yet) */
 	SswSnap<R> snap;
 	if constexpr (TRACK)
 		ssw_snap_init<R>(snap, reinterpret_cast<uint4*>(smem + (size_t)(share ? 1 : nwarps) * (size_t)(n + 1) * 32 * S), (int)threadIdx.x);
-	uint32_t blk_acc = 0, blk_done = 0;                 /* CM == 2: this lane's maximum of its current block, and of its last finished one */
+	/* block mode: this lane's maximum (CM == 3: of its E samples, starting below every sample) of its current block, and of
+	 * its last finished one */
+	uint32_t blk_acc = CM == 3 ? 0x80008000u : 0u, blk_done = 0;
 
 	for (int body = 0; body < n_body; ++body) {
-		uint32_t cmv[U];                                /* per step: outC, or in block mode the maximum over this lane's own rows */
+		uint32_t cmv[U];                                /* per step: outC, or with CM == 2 the maximum over this lane's own rows */
 		if (TRACK && (body & (SSW_FLOOR_PERIOD - 1)) == 0) {
 			/* lower bound of the group's final maximum: a lane value below it can never be the best cell, so the lane's
 			 * running best is raised to (bound - 1) and such values no longer trigger the bookkeeping */
@@ -486,7 +492,7 @@ ssw_fill_kernel(const SswItem* __restrict__ items, int n_items,
 			/* values crossing the lane boundary */
 			const uint32_t inH = __shfl_up_sync(FULL, outH, 1, G) * top_keep;
 			const uint32_t inF = __shfl_up_sync(FULL, outF, 1, G) * top_keep;
-			const uint32_t inC = CM == 2 ? 0u : __shfl_up_sync(FULL, outC, 1, G) * top_keep;   /* block mode: outC unused */
+			const uint32_t inC = BLK ? 0u : __shfl_up_sync(FULL, outC, 1, G) * top_keep;   /* block mode: outC unused */
 
 			/* reference letter of this lane's scan position and its profile rows */
 			int letter = (int)lptr[DIR * j];
@@ -551,6 +557,33 @@ ssw_fill_kernel(const SswItem* __restrict__ items, int n_items,
 				blk_acc = __vimax3_s16x2(blk_acc, cmv[4], cmv[5]);
 				blk_acc = __vimax3_s16x2(blk_acc, cmv[6], cmv[7]);
 			}
+		}
+		if (CM == 3) {
+			/* Bounded block words (DESIGN 2): no per-step maximum at all.  After step 7 E holds E(r, c + 1) of this lane's last
+			 * column c of the body, and in every row H(r, c') <= E(r, c + 1) + gapO + (c - c') gapE for the body's columns c',
+			 * while E(r, c + 1) <= H(r, c) - gapE.  So the maximum of E over the lane's rows, once per body, bounds the maxima
+			 * of the body's columns from above (+ gapO + 7 gapE) and the maximum of column c from below (+ gapE).  A body
+			 * that straddles a block boundary (step js in 1..7) is credited to both blocks: the upper bound holds for both, the
+			 * lower one for the later block only, which the resolve accounts for. */
+			uint32_t e;
+			if (R >= 3) {
+				e = __vimax3_s16x2(E[0], E[1], E[2]);
+#pragma unroll
+				for (int k = 3; k + 1 < R; k += 2) e = __vimax3_s16x2(e, E[k], E[k + 1]);
+				if (((R - 3) & 1) != 0) e = __vmaxs2(e, E[R - 1]);
+			} else e = R == 2 ? __vmaxs2(E[0], E[1]) : E[0];
+			constexpr int BODIES = SSW_CM_BLOCK / U;
+			const int bm = body % BODIES;
+			if (bm < G / U) {
+				const int js = t + 1 - U * bm;
+				if (js >= 1 && js <= U) { blk_done = __vmaxs2(blk_acc, e); blk_acc = js < U ? e : 0x80008000u; }
+				else blk_acc = __vmaxs2(blk_acc, e);
+				if (bm == G / U - 1) {
+					const uint32_t v = ssw_group_max<G>(blk_done);
+					const int c0 = sL + U - SSW_CM_BLOCK;
+					if (t == 0 && it.cm_off != SSW_CM_NONE && c0 >= it.p0 && c0 < it.p1) colmax[it.cm_off + c0 / SSW_CM_BLOCK] = v;
+				}
+			} else blk_acc = __vmaxs2(blk_acc, e);
 		}
 		if (TERM) {
 			/* reverse pass: stop after the first column whose maximum equals score1 (ssw.c:339/:541) */

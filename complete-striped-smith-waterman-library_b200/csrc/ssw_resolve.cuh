@@ -174,13 +174,95 @@ ssw_resolve_best_block_kernel(const SswAlnDesc* __restrict__ alns, int n_aln, co
 	                                        : ssw_refill_item(d, items, 0, 0);
 }
 
-/* stage 1: `best` holds the re-fill record of stage 0's block, one per alignment */
+/* ---- bounded block words (fill kernel CM == 3) ----
+ * The word of block b is w(b), and w(b) + gapE <= M(b) <= U(b) = w(b) + gapO + 7 gapE (DESIGN 2; the lower bound of a loop body
+ * that straddles two blocks belongs to the later one, so L(b) = w(b) + gapE <= max(M(b), M(b + 1))).  The exact best cell needs
+ * single columns only in the blocks C1 = {b : U(b) >= max(T1, 1)}, T1 = max_b L(b) <= score1, and the second-best scan only in
+ * the allowed blocks C2 = {b : U(b) >= max(T2, 1)} (stage 1) besides the window edges and the byte-row zone.  Each stage lists
+ * an alignment's candidates in block order in cand[idx * cap ...] and their number in cnt (-1: more than cap; the alignment
+ * is then resolved from exact words of its pair-task, ssw_engine.cu).  The host turns the counts into offsets, and
+ * ssw_bound_emit_kernel writes one re-fill item per candidate. */
+struct SswBound { int gapO, gapE, cap; };
+#define SSW_BOUND_CAP 256       /* default cap of the candidates per alignment and stage */
+
+/* blocks b of a row of n_blk words with w(b) >= thr that lie entirely outside [e1, e2), in block order, into out[< cap];
+ * returns their number (all of them, also beyond cap) */
+__device__ static __forceinline__ int ssw_bound_list(const uint32_t* __restrict__ w, int h, int n_blk, int ref_len, int thr,
+                                                     int e1, int e2, int32_t* __restrict__ out, int cap, int lane)
+{
+	int n = 0;
+	for (int b0 = 0; b0 < n_blk; b0 += 32) {
+		const int b = b0 + lane;
+		bool c = false;
+		if (b < n_blk) {
+			const int bs = b * SSW_CM_BLOCK, be = min(bs + SSW_CM_BLOCK, ref_len);
+			c = (be <= e1 || bs >= e2) && half_of(w[b], h) >= thr;
+		}
+		const unsigned m = __ballot_sync(0xffffffffu, c);
+		const int k = n + __popc(m & ((1u << lane) - 1u));
+		if (c && k < cap) out[k] = b;
+		n += __popc(m);
+	}
+	return n;
+}
+
+/* stage 0 of the bounded words: the C1 candidates of every alignment */
 template <int DUMMY = 0>
+__global__ void __launch_bounds__(SSW_RESOLVE_THREADS)
+ssw_bound_best_kernel(const SswAlnDesc* __restrict__ alns, int n_aln, const uint32_t* __restrict__ words, SswBound bd,
+                      int32_t* __restrict__ cand, int32_t* __restrict__ cnt)
+{
+	constexpr unsigned FULL = 0xffffffffu;
+	const int lane = threadIdx.x & 31;
+	const int idx = (int)blockIdx.x * (SSW_RESOLVE_THREADS / 32) + (threadIdx.x >> 5);
+	if (idx >= n_aln) return;
+	const SswAlnDesc d = alns[idx];
+	int n = 0;
+	if (d.cm_off != SSW_CM_NONE && d.n_items > 0) {
+		const uint32_t* w = words + d.cm_off;
+		const int n_blk = (d.ref_len + SSW_CM_BLOCK - 1) / SSW_CM_BLOCK;
+		int wm = -32768;
+		for (int b = lane; b < n_blk; b += 32) wm = max(wm, half_of(w[b], d.half));
+#pragma unroll
+		for (int off = 16; off >= 1; off >>= 1) wm = max(wm, __shfl_xor_sync(FULL, wm, off));
+		const int t1 = max(wm + bd.gapE, 1);
+		n = ssw_bound_list(w, d.half, n_blk, d.ref_len, t1 - bd.gapO - 7 * bd.gapE, 0, 0, cand + (int64_t)idx * bd.cap, bd.cap, lane);
+	}
+	if (lane == 0) cnt[idx] = n > bd.cap ? -1 : n;
+}
+
+/* one re-fill item per listed candidate block at off[idx] + k (cm != 0: with one column word each, at that slot of the scratch) */
+template <int DUMMY = 0>
+__global__ void __launch_bounds__(SSW_RESOLVE_THREADS)
+ssw_bound_emit_kernel(const SswAlnDesc* __restrict__ alns, int n_aln, const SswItem* __restrict__ items, const int32_t* __restrict__ cand,
+                      int cap, const int32_t* __restrict__ cnt, const int32_t* __restrict__ off, int cm, SswItem* __restrict__ out)
+{
+	const int lane = threadIdx.x & 31;
+	const int idx = (int)blockIdx.x * (SSW_RESOLVE_THREADS / 32) + (threadIdx.x >> 5);
+	if (idx >= n_aln) return;
+	const SswAlnDesc d = alns[idx];
+	const int n = cnt[idx];
+	for (int k = lane; k < n; k += 32) {
+		const int c0 = cand[(int64_t)idx * cap + k] * SSW_CM_BLOCK;
+		SswItem it = ssw_refill_item(d, items, c0, min(c0 + SSW_CM_BLOCK, d.ref_len));
+		const int64_t slot = (int64_t)off[idx] + k;
+		if (cm) it.cm_off = slot * SSW_CM_BLOCK - it.p0;
+		out[slot] = it;
+	}
+}
+
+/* Stage 1.  Exact words (BOUND false): `best` holds the re-fill record of stage 0's block, one per alignment.  Bounded words
+ * (BOUND true): `best` holds the re-fill records of the alignment's C1 candidates at [off1[idx], off1[idx] + cnt1[idx]), folded
+ * here in the same order as the item records of ssw_resolve_kernel (blocks are disjoint, so ties go to the first block); the
+ * third slot stays dead, and the C2 candidates of the second-best scan go to cand / cnt2 (ssw_bound_list). */
+template <bool BOUND = false>
 __global__ void __launch_bounds__(SSW_RESOLVE_THREADS)
 ssw_resolve_blocks_kernel(const SswAlnDesc* __restrict__ alns, int n_aln,
                           const SswItemBest* __restrict__ best, const uint32_t* __restrict__ blkmax,
                           const SswItem* __restrict__ items, SswFillResult* __restrict__ out,
-                          SswItem* __restrict__ refill_items, int32_t* __restrict__ refill_c0)
+                          SswItem* __restrict__ refill_items, int32_t* __restrict__ refill_c0,
+                          const int32_t* __restrict__ cnt1 = nullptr, const int32_t* __restrict__ off1 = nullptr,
+                          SswBound bd = SswBound{0, 0, 0}, int32_t* __restrict__ cand = nullptr, int32_t* __restrict__ cnt2 = nullptr)
 {
 	constexpr unsigned FULL = 0xffffffffu;
 	const int lane = threadIdx.x & 31;
@@ -189,8 +271,25 @@ ssw_resolve_blocks_kernel(const SswAlnDesc* __restrict__ alns, int n_aln,
 	const SswAlnDesc d = alns[idx];
 	const int h = d.half;
 
-	const SswItemBest bc = best[idx];
-	int sc = bc.score[h], pos = bc.pos[h], row = bc.row[h];
+	int sc = 0, pos = 0, row = 0;
+	if (BOUND) {
+		pos = 0x7fffffff; row = 0x7fffffff;
+		const int n1 = cnt1[idx];
+		for (int k = lane; k < n1; k += 32) {
+			const SswItemBest b = best[off1[idx] + k];
+			const int s = b.score[h], p = b.pos[h], rr = b.row[h];
+			if (s > 0 && (s > sc || (s == sc && (p < pos || (p == pos && rr < row))))) { sc = s; pos = p; row = rr; }
+		}
+#pragma unroll
+		for (int off = 16; off >= 1; off >>= 1) {
+			const int o_sc = __shfl_xor_sync(FULL, sc, off);
+			const int o_pos = __shfl_xor_sync(FULL, pos, off), o_row = __shfl_xor_sync(FULL, row, off);
+			if (o_sc > sc || (o_sc == sc && (o_pos < pos || (o_pos == pos && o_row < row)))) { sc = o_sc; pos = o_pos; row = o_row; }
+		}
+	} else {
+		const SswItemBest bc = best[idx];
+		sc = bc.score[h]; pos = bc.pos[h]; row = bc.row[h];
+	}
 	if (sc <= 0) { sc = 0; pos = 0; row = 0; }
 
 	SswFillResult r;
@@ -200,7 +299,7 @@ ssw_resolve_blocks_kernel(const SswAlnDesc* __restrict__ alns, int n_aln,
 	if (sc >= d.limit) { r.overflow = d.word ? 2 : 1; if (!d.word) r.score = 255; }
 
 	int slots[SSW_REFILL_SLOTS] = {-1, -1, -1, -1};     /* block ids; the zone slot: its first column */
-	int zone_end = 0;
+	int zone_end = 0, n2 = 0;
 	if (sc > 0 && !r.overflow && d.cm_off != SSW_CM_NONE && d.n_items > 0) {
 		const int e1 = max(pos - d.mask_len, 0);
 		const int e2 = min(pos + d.mask_len, d.ref_len) + (d.word ? 0 : 1);
@@ -209,7 +308,20 @@ ssw_resolve_blocks_kernel(const SswAlnDesc* __restrict__ alns, int n_aln,
 		 * pair-task's row are those of its items */
 		const uint32_t* bm = blkmax + d.cm_off;
 		const int n_blk = (d.ref_len + SSW_CM_BLOCK - 1) / SSW_CM_BLOCK;
+		if (BOUND) {
+			/* T2 = max L(b) over the fully allowed blocks b whose successor is fully allowed too (the lower bound of a body that
+			 * straddles into b + 1 belongs to b + 1), so T2 <= the largest fully allowed block maximum; only v > 0 can win */
+			int t2 = 1;
+			for (int b = lane; b + 1 < n_blk; b += 32) {
+				const int bs = b * SSW_CM_BLOCK, be = min(bs + 2 * SSW_CM_BLOCK, d.ref_len);
+				if (be <= e1 || bs >= e2) t2 = max(t2, half_of(bm[b], h) + bd.gapE);
+			}
+#pragma unroll
+			for (int off = 16; off >= 1; off >>= 1) t2 = max(t2, __shfl_xor_sync(FULL, t2, off));
+			n2 = ssw_bound_list(bm, h, n_blk, d.ref_len, t2 - bd.gapO - 7 * bd.gapE, e1, e2, cand + (int64_t)idx * bd.cap, bd.cap, lane);
+		}
 		int vb = 0, bb = 0x7fffffff;
+		if (!BOUND)
 		for (int b = lane; b < n_blk; b += 32) {
 			const int bs = b * SSW_CM_BLOCK, be = min(bs + SSW_CM_BLOCK, d.ref_len);
 			if (be <= e1 || bs >= e2) {
@@ -228,6 +340,7 @@ ssw_resolve_blocks_kernel(const SswAlnDesc* __restrict__ alns, int n_aln,
 		if (vb > 0) slots[2] = bb;
 	}
 	if (lane == 0) out[idx] = r;
+	if (BOUND && lane == 0) cnt2[idx] = n2 > bd.cap ? -1 : n2;
 	if (lane < SSW_REFILL_SLOTS) {
 		const int b = slots[lane];
 		const int64_t slot = (int64_t)idx * SSW_REFILL_SLOTS + lane;
@@ -244,10 +357,13 @@ ssw_resolve_blocks_kernel(const SswAlnDesc* __restrict__ alns, int n_aln,
 }
 
 /* stage 2: fold the re-filled ranges (single column maxima) into the second-best candidate of stage 1 */
+/* Bounded words: the C2 candidates (block ids cand[idx * cap + k], k < cnt2[idx]; column words at off2[idx] + k of cm2) as well. */
 template <int DUMMY = 0>
 __global__ void __launch_bounds__(SSW_RESOLVE_THREADS)
 ssw_resolve_refill_kernel(const SswAlnDesc* __restrict__ alns, int n_aln, const int32_t* __restrict__ refill_c0,
-                          const uint32_t* __restrict__ refill_cm, SswFillResult* __restrict__ out)
+                          const uint32_t* __restrict__ refill_cm, SswFillResult* __restrict__ out,
+                          const int32_t* __restrict__ cand = nullptr, int cap = 0, const int32_t* __restrict__ cnt2 = nullptr,
+                          const int32_t* __restrict__ off2 = nullptr, const uint32_t* __restrict__ cm2 = nullptr)
 {
 	constexpr unsigned FULL = 0xffffffffu;
 	const int lane = threadIdx.x & 31;
@@ -270,6 +386,18 @@ ssw_resolve_refill_kernel(const SswAlnDesc* __restrict__ alns, int n_aln, const 
 			const int c = c0 + j;
 			if (c < e1 || c >= e2) {
 				const int v = half_of(refill_cm[slot * SSW_CM_BLOCK + j], h);
+				if (ssw_second_better(v, c, v2, i2)) { v2 = v; i2 = c; }
+			}
+		}
+	}
+	const int n2 = cnt2 ? cnt2[idx] : 0;
+	for (int k = 0; k < n2; ++k) {
+		const int c0 = cand[(int64_t)idx * cap + k] * SSW_CM_BLOCK, c1 = min(c0 + SSW_CM_BLOCK, d.ref_len);
+		const uint32_t* w = cm2 + (int64_t)(off2[idx] + k) * SSW_CM_BLOCK;
+		for (int j = lane; c0 + j < c1; j += 32) {
+			const int c = c0 + j;
+			if (c < e1 || c >= e2) {
+				const int v = half_of(w[j], h);
 				if (ssw_second_better(v, c, v2, i2)) { v2 = v; i2 = c; }
 			}
 		}

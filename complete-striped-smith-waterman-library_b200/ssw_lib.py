@@ -48,7 +48,8 @@ class EngineTiming(ct.Structure):
                 ("traceback_ms", ct.c_float), ("total_ms", ct.c_float),
                 ("fill_forward_launches", ct.c_int64), ("other_launches", ct.c_int64),
                 ("cells_forward", ct.c_int64), ("byte_overflows", ct.c_int64),
-                ("grid_cols_planned", ct.c_int64), ("grid_cols_useful", ct.c_int64), ("leftover_pairs", ct.c_int64)]
+                ("grid_cols_planned", ct.c_int64), ("grid_cols_useful", ct.c_int64), ("leftover_pairs", ct.c_int64),
+                ("block_refills", ct.c_int64), ("block_exact", ct.c_int64)]
 
 
 # numpy view of ssw_batch_result (36 bytes)

@@ -283,6 +283,9 @@ typedef struct {
 	int64_t grid_cols_planned;   /* group-columns the fill launches sweep: over the warps, groups per warp x the longest reference of the warp */
 	int64_t grid_cols_useful;    /* of these, columns of a group's own reference; useful / planned = the planned sweep efficiency */
 	int64_t leftover_pairs;      /* ssw_engine_search(_all): pairs outside the device-planned grid (general path, selection on the host) */
+	/* bounded block words of the forward fill ("cm_block" -1 or 2) */
+	int64_t block_refills;       /* candidate blocks re-filled to resolve the best cell (C1) and the second best (C2) */
+	int64_t block_exact;         /* alignments with more than 256 candidate blocks in a stage, resolved from exact block maxima of their pair-task */
 } ssw_engine_timing;
 int ssw_engine_last_timing(const ssw_engine* e, ssw_engine_timing* t);
 /* Column maxima of the engine's last forward fill launch, for tests: packed s16x2 words (the two alignments of a pair-task),
@@ -296,8 +299,10 @@ int64_t ssw_engine_last_colmax(ssw_engine* e, uint32_t* out, int64_t n_words);
  * its own set; e == NULL addresses the engines behind ssw_align / ssw_align_batch(NULL, ...) (present and future).
  *   "chunk"         reference chunk length in columns of the fill kernel (0 = automatic)
  *   "small_chunk"   the same for launches too small to fill the device (0 = automatic)
- *   "cm_block"      column maxima of the forward fill: -1 automatic, 0 one word per column, 1 one word per 64 columns
- *                   (+ re-fill of the blocks whose single columns matter) wherever the reference can be chunked
+ *   "cm_block"      column maxima of the forward fill: -1 automatic (bounded block words for long references), 0 one word per
+ *                   column, 1 the exact maximum of every 64 columns (+ re-fill of the blocks whose single columns matter) wherever
+ *                   the reference can be chunked, 2 bounded block words (a bracket of every 64 columns' maximum, + re-fill of the
+ *                   blocks the bracket cannot rule out: DESIGN 2) wherever the reference can be chunked.  Same results in every mode.
  *   "cm_budget_mb"  cap of the column-maximum scratch per launch in MiB (0 = a share of the free device memory)
  *   "inst"          force forward kernel instance i (rows-per-lane / lanes-per-group table of the engine; -1 = automatic)
  *   "latency_cols"  passes over at most this many reference columns use the 32-lane instances (0 = never)
