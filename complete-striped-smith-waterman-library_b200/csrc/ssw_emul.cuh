@@ -19,7 +19,8 @@
 #define SSW_EMUL_THREADS (SSW_EMUL_WARPS * 32)
 
 struct SswEmulTask {
-	int32_t q_off, q_len, q_rev;   /* query rows: code[q_off + row], or the reversed prefix code[q_off + q_len-1-row] */
+	int32_t q_off, q_len, q_rev;   /* query rows: code[q_off + row], or the reversed prefix code[q_off + q_len-1-row] (query
+	                                * profiles: q_off counts rows of n scores) */
 	int32_t ref_len;               /* columns scanned: [0, ref_len) forward, ref_len-1 .. 0 when dir == 1 */
 	int64_t ref_off;               /* offset of reference column 0 in the padded reference array */
 	int32_t dir, word, terminate, bias, mask_len, pad_;
@@ -49,7 +50,7 @@ ssw_emul_kernel(const SswEmulTask* __restrict__ tasks, int n_tasks,
 	int32_t* Hm = E + cells;
 	uint16_t* cm = cmax + T.cm_off;
 	const int8_t* ref = refs + T.ref_off;
-	const int8_t* q = qcodes + T.q_off;
+	const int8_t* q = qcodes + (mat ? (int64_t)T.q_off : (int64_t)T.q_off * n);   /* mat == nullptr: n-score profile rows */
 	for (int i = lane; i < 4 * cells; i += 32) Hs[i] = 0;
 	__syncwarp();
 
@@ -71,8 +72,8 @@ ssw_emul_kernel(const SswEmulTask* __restrict__ tasks, int n_tasks,
 				int p;
 				if (row >= T.q_len) p = T.word ? 0 : T.bias;
 				else {
-					const int code = (int)q[T.q_rev ? T.q_len - 1 - row : row];
-					const int m = (int)mat[letter * n + code];
+					const int qr = T.q_rev ? T.q_len - 1 - row : row;
+					const int m = mat ? (int)mat[letter * n + (int)q[qr]] : (int)q[(int64_t)qr * n + letter];
 					p = T.word ? m : ((m + T.bias) & 0xff);
 				}
 				int h;

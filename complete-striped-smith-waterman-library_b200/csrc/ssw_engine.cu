@@ -185,6 +185,10 @@ struct ssw_engine {
 	int64_t cached_ref_len = -1;     /* ssw_engine_set_pair: length and content hash of the single resident reference (-1: none) */
 	uint64_t cached_ref_hash = 0;
 	SswDevBuf d_q, d_r, d_mat;
+	/* query profiles (ssw_engine_set_sequences_pssm): d_q holds n scores per row and q_off counts rows; pssm_n is that n (0: query
+	 * codes are resident).  Per query: the byte bias max(0, -min P) and the largest score, as ssw_init derives them from a matrix. */
+	int pssm_n = 0;
+	std::vector<int32_t> q_bias, q_max;
 
 	/* scratch */
 	SswDevBuf d_items, d_bests, d_alns, d_res, d_colmax, d_tb, d_bnd, d_park, d_emul, d_grid, d_out, d_sync;
@@ -214,6 +218,8 @@ struct ssw_engine {
 	}
 
 	int upload_refs(int n);
+	/* the matrix argument of the kernels: nullptr tells them that d_q holds query profiles */
+	const int8_t* mat_arg() const { return pssm_n ? nullptr : d_mat.as<int8_t>(); }
 	int run_fill(const std::vector<SswItem>& items, int inst, int dir, int cm_mode, int share, const ssw_batch_params& P, float* ms_acc);
 };
 
@@ -250,8 +256,8 @@ static int fill_items_per_cta(int inst, int n)
 	return visit_inst(inst, [n](auto t) { using T = decltype(t); return fill_shape<T::R>(n, 1, +1).warps * (32 / T::G); });
 }
 
-template <int G, int R>
-static int launch_fill(ssw_engine* e, const FillPtrs& fp, int n_items, int dir, int cm_mode, int share, const ssw_batch_params& P)
+template <int G, int R, bool PSSM>
+static int launch_fill_src(ssw_engine* e, const FillPtrs& fp, int n_items, int dir, int cm_mode, int share, const ssw_batch_params& P)
 {
 	const FillShape sh = fill_shape<R>(P.n, share, dir, !(dir > 0 && cm_mode >= 2));
 	if (sh.smem > 220 * 1024) { fprintf(stderr, "[libssw-b200] alphabet of %d letters is too large for this query length\n", P.n); return -2; }
@@ -259,7 +265,7 @@ static int launch_fill(ssw_engine* e, const FillPtrs& fp, int n_items, int dir, 
 	const int grid = (n_items + per_cta - 1) / per_cta;
 	const int8_t* q = e->d_q.as<int8_t>();
 	const int8_t* r = e->d_r.as<int8_t>();
-	const int8_t* mat = e->d_mat.as<int8_t>();
+	const int8_t* mat = e->mat_arg();
 	auto go = [&](auto kern) {
 		if (ssw_ensure_dyn_smem(reinterpret_cast<const void*>(kern), sh.smem)) return -1;
 		ssw_launch(kern, dim3(grid), dim3(sh.warps * 32), sh.smem, e->stream, fp.items, n_items, q, r, mat, (int)P.n,
@@ -268,21 +274,28 @@ static int launch_fill(ssw_engine* e, const FillPtrs& fp, int n_items, int dir, 
 		return 0;
 	};
 	if (dir < 0) {   /* reverse: one alignment per warp, early termination */
-		if constexpr (G == 32) return go(ssw_fill_kernel<G, R, -1, 0, true, SSW_FILL_WARPS, false>);
+		if constexpr (G == 32) return go(ssw_fill_kernel<G, R, -1, 0, true, SSW_FILL_WARPS, false, PSSM>);
 		return -2;
 	}
 	/* forward: column maxima per column or per block */
 	if (sh.warps == 8) {
 		if constexpr (R >= 16) {
-			if (cm_mode == 2) return go(ssw_fill_kernel<G, R, 1, 2, false, 8, false>);
-			if (cm_mode == 3) return go(ssw_fill_kernel<G, R, 1, 3, false, 8, false>);
-			return fp.arm ? go(ssw_fill_kernel<G, R, 1, 1, false, 8, true>) : go(ssw_fill_kernel<G, R, 1, 1, false, 8, false>);
+			if (cm_mode == 2) return go(ssw_fill_kernel<G, R, 1, 2, false, 8, false, PSSM>);
+			if (cm_mode == 3) return go(ssw_fill_kernel<G, R, 1, 3, false, 8, false, PSSM>);
+			return fp.arm ? go(ssw_fill_kernel<G, R, 1, 1, false, 8, true, PSSM>) : go(ssw_fill_kernel<G, R, 1, 1, false, 8, false, PSSM>);
 		}
 		return -2;
 	}
-	if (cm_mode == 2) return go(ssw_fill_kernel<G, R, 1, 2, false, SSW_FILL_WARPS, false>);
-	if (cm_mode == 3) return go(ssw_fill_kernel<G, R, 1, 3, false, SSW_FILL_WARPS, false>);
-	return fp.arm ? go(ssw_fill_kernel<G, R, 1, 1, false, SSW_FILL_WARPS, true>) : go(ssw_fill_kernel<G, R, 1, 1, false, SSW_FILL_WARPS, false>);
+	if (cm_mode == 2) return go(ssw_fill_kernel<G, R, 1, 2, false, SSW_FILL_WARPS, false, PSSM>);
+	if (cm_mode == 3) return go(ssw_fill_kernel<G, R, 1, 3, false, SSW_FILL_WARPS, false, PSSM>);
+	return fp.arm ? go(ssw_fill_kernel<G, R, 1, 1, false, SSW_FILL_WARPS, true, PSSM>) : go(ssw_fill_kernel<G, R, 1, 1, false, SSW_FILL_WARPS, false, PSSM>);
+}
+
+/* the fill kernels' instances for query profiles (PSSM) or query codes */
+template <int G, int R>
+static int launch_fill(ssw_engine* e, const FillPtrs& fp, int n_items, int dir, int cm_mode, int share, const ssw_batch_params& P)
+{
+	return e->pssm_n ? launch_fill_src<G, R, true>(e, fp, n_items, dir, cm_mode, share, P) : launch_fill_src<G, R, false>(e, fp, n_items, dir, cm_mode, share, P);
 }
 
 static int dispatch_fill(ssw_engine* e, int inst, const FillPtrs& fp, int n_items, int dir, int cm_mode, int share, const ssw_batch_params& P)
@@ -460,27 +473,46 @@ static int check_offsets(const char* what, int32_t n, const int64_t* off, int64_
 #define SSW_MAX_QUERY_LETTERS ((int64_t)0x7fffffff - 64)                        /* SswQuery.off is 32 bits */
 #define SSW_MAX_REF_LEN ((int64_t)0x7fffffff - 4 * SSW_REF_PAD - 64)            /* SswItem.ref_len, scan positions */
 
+/* pssm_n > 0: the queries are position-specific profiles of pssm_n scores per row (query_off counts rows); 0: query codes. */
 static int set_sequences_impl(ssw_engine* e,
                               int32_t n_queries, const int8_t* queries, const int64_t* query_off,
-                              int32_t n_refs, const int8_t* refs, const int64_t* ref_off)
+                              int32_t n_refs, const int8_t* refs, const int64_t* ref_off, int32_t pssm_n = 0)
 {
 	if (!e || n_queries < 0 || n_refs < 0 || (n_queries && (!queries || !query_off)) || (n_refs && (!refs || !ref_off))) return -1;
-	if (check_offsets("query", n_queries, query_off, SSW_MAX_QUERY_LETTERS, SSW_MAX_QUERY_LETTERS)) return -1;
+	if (pssm_n < 0 || pssm_n > 64) { fprintf(stderr, "[libssw-b200] profiles of %d letters: 1 .. 64 supported\n", pssm_n); return -1; }
+	/* profiles: the banded traceback addresses a row's scores within its query in 32 bits */
+	if (check_offsets("query", n_queries, query_off, SSW_MAX_QUERY_LETTERS, pssm_n ? 0x7fffffff / pssm_n - 64 : SSW_MAX_QUERY_LETTERS)) return -1;
 	if (check_offsets("reference", n_refs, ref_off, (int64_t)1 << 46, SSW_MAX_REF_LEN)) return -1;
 	SSW_CUDA_OK(cudaSetDevice(e->device));
 	e->n_q = n_queries; e->n_r = n_refs;
 	e->from_text = false;
 	e->cached_ref_len = -1;
 	e->grid_arm_ok = true;
-	const int64_t qb = n_queries ? query_off[n_queries] : 0, rb = n_refs ? ref_off[n_refs] : 0;
+	e->pssm_n = pssm_n;
+	const int64_t width = pssm_n ? pssm_n : 1;
+	const int64_t qb = (n_queries ? query_off[n_queries] : 0) * width, rb = n_refs ? ref_off[n_refs] : 0;
 	if (n_queries) e->q_off.assign(query_off, query_off + n_queries + 1); else e->q_off.assign(1, 0);
 	e->h_q.assign(queries, queries + qb);
 	if (n_refs) e->h_r_off.assign(ref_off, ref_off + n_refs + 1); else e->h_r_off.assign(1, 0);
 	e->h_r.assign(refs, refs + rb);
 	e->r_len.resize(n_refs);
 	for (int i = 0; i < n_refs; ++i) e->r_len[i] = (int32_t)(ref_off[i + 1] - ref_off[i]);
-	if (e->d_q.ensure(e->h_q.size() + 16)) return -1;
+	e->q_bias.clear(); e->q_max.clear();
+	if (pssm_n) {
+		/* what ssw_init derives from the matrix of a profile (ssw.c:834-838): the byte bias, and the largest score for the word guard */
+		e->q_bias.resize((size_t)n_queries); e->q_max.resize((size_t)n_queries);
+		for (int32_t q = 0; q < n_queries; ++q) {
+			int lo = 0, hi = 0;
+			if (query_off[q + 1] > query_off[q]) { lo = 127; hi = -128; }
+			for (int64_t i = query_off[q] * width; i < query_off[q + 1] * width; ++i) { lo = std::min<int>(lo, queries[i]); hi = std::max<int>(hi, queries[i]); }
+			e->q_bias[q] = std::max(0, -lo); e->q_max[q] = hi;
+		}
+	}
+	/* behind the last query a few zero bytes (profiles: two rows), so that no read of a row just past a query leaves the buffer */
+	const size_t tail = pssm_n ? (size_t)(16 + 2 * pssm_n) : 16;
+	if (e->d_q.ensure(e->h_q.size() + tail)) return -1;
 	if (qb) SSW_CUDA_OK(cudaMemcpyAsync(e->d_q.p, e->h_q.data(), e->h_q.size(), cudaMemcpyHostToDevice, e->stream));
+	if (pssm_n) SSW_CUDA_OK(cudaMemsetAsync(e->d_q.as<int8_t>() + qb, 0, tail, e->stream));
 	e->padded_n = -1;           /* the null letter depends on the alphabet size given at align time */
 	return 0;
 }
@@ -491,6 +523,16 @@ extern "C" int ssw_engine_set_sequences(ssw_engine* e,
 {
 	try { return set_sequences_impl(e, n_queries, queries, query_off, n_refs, refs, ref_off); }
 	catch (const std::exception& ex) { fprintf(stderr, "[libssw-b200] ssw_engine_set_sequences: %s\n", ex.what()); return -1; }
+	catch (...) { return -1; }
+}
+
+extern "C" int ssw_engine_set_sequences_pssm(ssw_engine* e,
+                                             int32_t n_queries, const int8_t* pssm, const int64_t* query_off, int32_t n,
+                                             int32_t n_refs, const int8_t* refs, const int64_t* ref_off)
+{
+	if (n < 1) { fprintf(stderr, "[libssw-b200] ssw_engine_set_sequences_pssm: profiles of %d letters: 1 .. 64 supported\n", n); return -1; }
+	try { return set_sequences_impl(e, n_queries, pssm, query_off, n_refs, refs, ref_off, n); }
+	catch (const std::exception& ex) { fprintf(stderr, "[libssw-b200] ssw_engine_set_sequences_pssm: %s\n", ex.what()); return -1; }
 	catch (...) { return -1; }
 }
 
@@ -512,6 +554,7 @@ extern "C" int ssw_engine_set_pair(ssw_engine* e, const int8_t* read, int32_t re
 		}
 		SSW_CUDA_OK(cudaSetDevice(e->device));
 		e->n_q = 1;
+		e->pssm_n = 0;
 		e->q_off.assign(2, 0); e->q_off[1] = readLen;
 		e->h_q.assign(read, read + readLen);
 		if (e->d_q.ensure(e->h_q.size() + 16)) return -1;
@@ -533,6 +576,7 @@ static int set_sequences_packed_impl(ssw_engine* e, int32_t n_queries, const int
 	SSW_CUDA_OK(cudaSetDevice(e->device));
 	e->cached_ref_len = -1;
 	e->grid_arm_ok = true;
+	e->pssm_n = 0;
 	const int64_t qb = n_queries ? query_off[n_queries] : 0, rb = n_refs ? ref_off[n_refs] : 0;
 	e->n_q = n_queries; e->n_r = n_refs;
 	if (n_queries) e->q_off.assign(query_off, query_off + n_queries + 1); else e->q_off.assign(1, 0);
@@ -599,6 +643,7 @@ static int set_sequences_text_impl(ssw_engine* e,
 	SSW_CUDA_OK(cudaSetDevice(e->device));
 	e->cached_ref_len = -1;
 	e->grid_arm_ok = true;
+	e->pssm_n = 0;
 	const int64_t qb = n_queries ? query_off[n_queries] : 0, rb = n_refs ? ref_off[n_refs] : 0;
 	e->n_q = n_queries * (1 + rc); e->n_r = n_refs;
 	if (n_queries) e->q_off.assign(query_off, query_off + n_queries + 1); else e->q_off.assign(1, 0);
@@ -654,12 +699,20 @@ struct Aln {            /* one requested pair while it moves through the phases 
 	int32_t rev_score, rev_pos, rev_row;
 };
 
-/* scoring context of one call */
+/* scoring context of one call.  With query profiles resident the bias and the limits are those of each query (q_bias / q_max
+ * non-null); bias and max_mat are then the largest over the resident profiles, for the call-wide bounds. */
 struct Sem {
 	int bias, max_mat;
 	int limit_byte;     /* 255 - bias: a byte-semantics score >= this overflows (ssw.c:329) */
 	int limit_word;     /* 16-bit head-room guard */
 	bool has_byte, has_word;
+	const int32_t* q_bias = nullptr;
+	const int32_t* q_max = nullptr;
+	int bias_of(int32_t q) const { return q_bias ? q_bias[q] : bias; }
+	int limit_byte_of(int32_t q) const { return q_bias ? 255 - q_bias[q] : limit_byte; }
+	int limit_word_of(int32_t q) const { return q_max ? 32767 - std::max(q_max[q], 0) - 256 : limit_word; }
+	int limit_of(int32_t q, int word) const { return word ? limit_word_of(q) : limit_byte_of(q); }
+	int max_of(int32_t q) const { return q_max ? q_max[q] : max_mat; }
 };
 
 static inline int lp_of(int len, int word) { int g = word ? 8 : 16; return (len + g - 1) / g * g; }
@@ -667,10 +720,10 @@ static inline int lp_of(int len, int word) { int g = word ? 8 : 16; return (len 
 /* Does a forward result obtained with semantics `word` have to be replaced by the other semantics?
  *   byte result that overflowed -> word (ssw.c:883-886)
  *   word result computed first because an overflow was predicted, but the score fits a byte -> byte */
-static inline bool needs_other(const SswFillResult& r, int word, const Sem& S, bool word_first)
+static inline bool needs_other(const SswFillResult& r, int word, const Sem& S, bool word_first, int32_t q)
 {
 	if (!word) return r.overflow == 1 && S.has_word;
-	return word_first && S.has_byte && r.overflow == 0 && r.score < S.limit_byte;
+	return word_first && S.has_byte && r.overflow == 0 && r.score < S.limit_byte_of(q);
 }
 
 /* How the column maxima of the fill being resolved are stored (fill kernel CM mode), and -- block mode -- what the
@@ -872,13 +925,13 @@ static int resolve_forward(ssw_engine* e, std::vector<SswAlnDesc>& descs, const 
 	for (size_t i = 0; i < descs.size(); ++i) {
 		Aln& a = alns[desc_aln[i]];
 		a.fwd = res[i]; a.word = word;
-		if (!needs_other(res[i], word, S, word_first)) continue;
+		if (!needs_other(res[i], word, S, word_first, a.q)) continue;
 		/* the rows the alignment was filled on: a byte alignment filled on its word rows (byte_pad > 0, DESIGN 2) is the
 		 * word fill of its read, so its word result lies in the same column maxima and item bests */
 		if (lp_of(a.read_len, word) - (pad_reuse ? descs[i].byte_pad : 0) == lp_of(a.read_len, !word)) {
 			SswAlnDesc d = descs[i];
 			d.word = !word;
-			d.limit = d.word ? S.limit_word : S.limit_byte;
+			d.limit = S.limit_of(a.q, d.word);
 			d.byte_pad = 0;             /* the byte-row columns right of the mask window matter to byte semantics only */
 			alt.push_back(d);
 			alt_aln.push_back(desc_aln[i]);
@@ -1017,11 +1070,12 @@ static int run_strips(ssw_engine* e, const ssw_batch_params& P, const std::vecto
 		e->laps.start(e->stream);
 #define SSW_STRIPS_GO(DIR, TERM, SPLIT)                                                                                 \
 		do {                                                                                                            \
-			auto kern = ssw_fill_strips_kernel<SSW_STRIP_R, DIR, TERM, SPLIT>;                                          \
+			auto kern = e->pssm_n ? ssw_fill_strips_kernel<SSW_STRIP_R, DIR, TERM, SPLIT, true>                          \
+			                      : ssw_fill_strips_kernel<SSW_STRIP_R, DIR, TERM, SPLIT, false>;                         \
 			if (ssw_ensure_dyn_smem(reinterpret_cast<const void*>(kern), smem)) return -1;                              \
 			if (e->opt.carve && ssw_prefer_max_smem(reinterpret_cast<const void*>(kern))) return -1;                    \
 			ssw_launch(kern, dim3((unsigned)(tasks.size() * (size_t)parts)), dim3(nw * 32), smem, e->stream, (const SswStripTask*)e->d_items.as<SswStripTask>(), \
-			           (const int8_t*)e->d_q.as<int8_t>(), (const int8_t*)e->d_r.as<int8_t>(), (const int8_t*)e->d_mat.as<int8_t>(), (int)P.n, \
+			           (const int8_t*)e->d_q.as<int8_t>(), (const int8_t*)e->d_r.as<int8_t>(), e->mat_arg(), (int)P.n, \
 			           (int)P.gap_open, (int)P.gap_extend, e->d_colmax.as<uint32_t>(), e->d_bnd.as<uint32_t>(), e->d_park.as<uint32_t>(), \
 			           e->d_bests.as<SswItemBest>(), parts, e->d_sync.as<int>());                                       \
 		} while (0)
@@ -1049,7 +1103,6 @@ static int forward_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Al
 {
 	if (sel.empty()) return 0;
 	Trace tr;
-	const int limit = word ? S.limit_word : S.limit_byte;
 	struct Key { int inst; int32_t r; int32_t q; int32_t lp; int64_t idx; };
 	std::vector<Key> keys, long_keys;          /* long_keys: queries longer than one strip */
 	/* A pass over few columns cannot fill the device whatever its layout, so its duration is the latency of one group's
@@ -1109,7 +1162,7 @@ static int forward_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Al
 		}
 		const int rc = run_strips(e, P, reqs, +1, false, alns, &e->timing.fill_forward_ms,
 		                          [&](std::vector<SswAlnDesc>& descs, const std::vector<int64_t>& desc_aln) -> int {
-			for (SswAlnDesc& d : descs) { d.word = word; d.limit = limit; }
+			for (size_t j = 0; j < descs.size(); ++j) { descs[j].word = word; descs[j].limit = S.limit_of(alns[desc_aln[j]].q, word); }
 			return resolve_forward(e, descs, desc_aln, alns, word, S, word_first, refill);
 		});
 		if (rc) return rc;
@@ -1313,10 +1366,10 @@ static int forward_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Al
 				SswAlnDesc d;
 				memset(&d, 0, sizeof(d));
 				d.first_item = first_item; d.n_items = pl.n_chunks; d.half = h; d.ref_len = ref_len; d.read_len = X.read_len;
-				d.word = word; d.limit = limit; d.mask_len = X.mask_len; d.cm_off = (int64_t)cm_words; d.warm = pl.warm;
+				d.word = word; d.limit = S.limit_of(X.q, word); d.mask_len = X.mask_len; d.cm_off = (int64_t)cm_words; d.warm = pl.warm;
 				d.byte_pad = lp_of(X.read_len, word) - fill_lp(X.read_len);
 				rf_lp = std::max(rf_lp, lp_of(X.read_len, word));
-				if (dual && h == 1) { d.word = 1; d.limit = S.limit_word; }
+				if (dual && h == 1) { d.word = 1; d.limit = S.limit_word_of(X.q); }
 				descs.push_back(d);
 				desc_aln.push_back(h ? pt.b : pt.a);
 			}
@@ -1450,7 +1503,7 @@ static int emul_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Aln>&
 			T.ref_off = e->r_off[a.r];
 			T.dir = dir; T.word = w;
 			T.terminate = dir ? a.fwd.score : (w ? 65535 : 255);
-			T.bias = S.bias; T.mask_len = a.mask_len;
+			T.bias = S.bias_of(a.q); T.mask_len = a.mask_len;
 			const size_t st = 4 * (size_t)((T.q_len + L - 1) / L) * L;
 			const size_t cm = ((size_t)T.ref_len + 7) / 8 * 8;
 			if (!tasks.empty() && 4 * (state_words + st) + 2 * (cm_elems + cm) > budget) break;
@@ -1469,7 +1522,7 @@ static int emul_pass(ssw_engine* e, const ssw_batch_params& P, std::vector<Aln>&
 		e->laps.start(e->stream);
 		ssw_launch(ssw_emul_kernel, dim3(((int)tasks.size() + SSW_EMUL_WARPS - 1) / SSW_EMUL_WARPS), dim3(SSW_EMUL_THREADS), 0, e->stream,
 		           (const SswEmulTask*)reinterpret_cast<SswEmulTask*>(base + off_tasks), (int)tasks.size(),
-		           (const int8_t*)e->d_q.as<int8_t>(), (const int8_t*)e->d_r.as<int8_t>(), (const int8_t*)e->d_mat.as<int8_t>(), (int)P.n,
+		           (const int8_t*)e->d_q.as<int8_t>(), (const int8_t*)e->d_r.as<int8_t>(), e->mat_arg(), (int)P.n,
 		           (int)P.gap_open, (int)P.gap_extend, reinterpret_cast<int32_t*>(base), reinterpret_cast<uint16_t*>(base + off_cm),
 		           reinterpret_cast<SswFillResult*>(base + off_res));
 		SSW_CUDA_OK(cudaGetLastError());
@@ -1520,7 +1573,6 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 	if (P.flag != 0 || P.gap_open <= P.gap_extend || e->opt.chunk != 0) return 0;
 	if (!S.has_byte && !S.has_word) return 0;
 	const int word = S.has_byte ? 0 : 1;
-	const int limit = word ? S.limit_word : S.limit_byte;
 	const int n_q = e->n_q, n_r_all = e->n_r;
 	/* The references of the grid, in ascending order of their index: the device's tables hold these n_r sequences only and
 	 * number them 0 .. n_r - 1 (the selection kernel breaks ties by that number, which the ascending order keeps equivalent
@@ -1536,8 +1588,9 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 		const int len = (int)(e->q_off[q + 1] - e->q_off[q]);
 		qt[q].off = (int32_t)e->q_off[q]; qt[q].len = len; qt[q].lp = lp_of(std::max(len, 1), word);
 		qt[q].mask_len = P.mask_len < 0 ? len / 2 : P.mask_len;
+		qt[q].limit = S.limit_of(q, word);
 		if (len < 1) continue;
-		if (S.has_byte && S.has_word && (int64_t)len * std::max(S.max_mat, 0) >= 2 * (int64_t)S.limit_byte) continue;   /* word-first prediction: general path */
+		if (S.has_byte && S.has_word && (int64_t)len * std::max(S.max_of(q), 0) >= 2 * (int64_t)S.limit_byte_of(q)) continue;   /* word-first prediction: general path */
 		q_inst[q] = pick_inst(qt[q].lp, e->opt.force_inst);
 		if (q_inst[q] >= 0) order.push_back(q);
 	}
@@ -1703,7 +1756,7 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 				qps.push_back(pr);
 			}
 			SswGridArgs A;
-			A.n_qp = (int32_t)qps.size(); A.n_r = n_rt; A.n_r_pad = n_r_pad; A.word = word; A.limit = limit; A.cm_words_per_qp = cm_per_qp;
+			A.n_qp = (int32_t)qps.size(); A.n_r = n_rt; A.n_r_pad = n_r_pad; A.word = word; A.cm_words_per_qp = cm_per_qp;
 			A.arm_tail = 0;
 			if (arm_on) {
 				int lp_max = 0;
@@ -1914,7 +1967,7 @@ static int align_general(ssw_engine* e, const ssw_batch_params& P, const Sem& S,
 	 * other semantics must replace is re-resolved on the same matrix or, if the pad rows differ, re-filled. ---- */
 	std::vector<int64_t> byte_first, word_first, refill_word, refill_byte;
 	for (int64_t p = 0; p < n_pairs; ++p) {
-		const bool predict = S.has_byte && S.has_word && (int64_t)alns[p].read_len * std::max(S.max_mat, 0) >= 2 * (int64_t)S.limit_byte;
+		const bool predict = S.has_byte && S.has_word && (int64_t)alns[p].read_len * std::max(S.max_of(alns[p].q), 0) >= 2 * (int64_t)S.limit_byte_of(alns[p].q);
 		if (!S.has_byte || predict) word_first.push_back(p); else byte_first.push_back(p);
 	}
 	int rc = 0;
@@ -1950,7 +2003,7 @@ static int align_general(ssw_engine* e, const ssw_batch_params& P, const Sem& S,
 	for (int64_t p = 0; p < n_pairs; ++p) {
 		const Aln& a = alns[p];
 		if (a.word == 0 && a.fwd.overflow == 1) { null_result[p] = 1; continue; }    /* byte overflow without a word profile (ssw.c:887-890) */
-		if (!literal && a.word == 1 && S.has_byte && a.fwd.score >= S.limit_byte) e->timing.byte_overflows += 1;
+		if (!literal && a.word == 1 && S.has_byte && a.fwd.score >= S.limit_byte_of(a.q)) e->timing.byte_overflows += 1;
 	}
 
 	phase.lap("general: forward passes");
@@ -1965,7 +2018,7 @@ static int align_general(ssw_engine* e, const ssw_batch_params& P, const Sem& S,
 	{
 		/* begin search: literal kernel where the forward result came from it (saturating scores) or the regime demands it */
 		std::vector<int64_t> rev_fast, rev_lit;
-		for (int64_t p : need_begin) (literal || alns[p].fwd.score >= S.limit_word ? rev_lit : rev_fast).push_back(p);
+		for (int64_t p : need_begin) (literal || alns[p].fwd.score >= S.limit_word_of(alns[p].q) ? rev_lit : rev_fast).push_back(p);
 		rc = reverse_pass(e, P, alns, rev_fast);
 		if (rc) return rc;
 		rc = emul_pass(e, P, alns, rev_lit, 1, 1, S);
@@ -2005,7 +2058,7 @@ static int align_general(ssw_engine* e, const ssw_batch_params& P, const Sem& S,
 		SswTbTask t;
 		memset(&t, 0, sizeof(t));
 		t.ref_off = e->r_off[a.r] + r.ref_begin1;
-		t.read_off = e->q_off[a.q] + r.read_begin1;
+		t.read_off = (e->q_off[a.q] + r.read_begin1) * (e->pssm_n ? e->pssm_n : 1);
 		t.ref_len = r.ref_end1 - r.ref_begin1 + 1;
 		t.read_len = r.read_end1 - r.read_begin1 + 1;
 		t.score = r.score1;
@@ -2016,7 +2069,7 @@ static int align_general(ssw_engine* e, const ssw_batch_params& P, const Sem& S,
 	phase.lap("general: records");
 	/* ---- P3 ---- */
 	if (!tb.empty()) {
-		rc = ssw_traceback_run(e->stream, e->side, tb, e->d_q.as<int8_t>(), e->d_r.as<int8_t>(), e->d_mat.as<int8_t>(), P.n,
+		rc = ssw_traceback_run(e->stream, e->side, tb, e->d_q.as<int8_t>(), e->d_r.as<int8_t>(), e->mat_arg(), P.n,
 		                       P.gap_open, P.gap_extend, &e->d_tb, &e->timing.traceback_ms, &e->timing.other_launches, e->opt.tb_maxbw, e->opt.carve != 0, e->opt.tb_spec,
 		                       [&](size_t i, const uint32_t* words, int32_t len, int failed) -> int {
 			ssw_batch_result& r = results[tb_pair[i]];
@@ -2034,17 +2087,40 @@ static int align_general(ssw_engine* e, const ssw_batch_params& P, const Sem& S,
 	return 0;
 }
 
-/* scoring matrix on the device and the semantics it implies: bias = |min(mat)| for byte semantics (ssw.c:834-838) */
+/* The scoring source of a call: a matrix (params->mat) with sequences resident, none (NULL, params->n = the profiles' n) with query
+ * profiles resident.  Prints why not and returns false. */
+static bool scoring_args_ok(const ssw_engine* e, const ssw_batch_params* params, const char* what)
+{
+	if (!e || !params) { fprintf(stderr, "[libssw-b200] %s: no engine or no parameters\n", what); return false; }
+	if (e->pssm_n && params->mat) { fprintf(stderr, "[libssw-b200] %s: query profiles are resident: params->mat must be NULL\n", what); return false; }
+	if (e->pssm_n && params->n != e->pssm_n) {
+		fprintf(stderr, "[libssw-b200] %s: the resident query profiles have %d letters, params->n is %d\n", what, e->pssm_n, params->n);
+		return false;
+	}
+	if (!e->pssm_n && !params->mat) { fprintf(stderr, "[libssw-b200] %s: no scoring matrix (params->mat is NULL) and no query profiles resident\n", what); return false; }
+	return true;
+}
+
+/* scoring matrix on the device and the semantics it implies: bias = |min(mat)| for byte semantics (ssw.c:834-838).  Query profiles:
+ * each query has its own bias and limits (taken at upload); bias and max_mat are their largest values, for the call-wide bounds. */
 static int prepare_scoring(ssw_engine* e, const ssw_batch_params& P, Sem* out)
 {
 	Sem& S = *out;
+	S.has_byte = P.score_size == 0 || P.score_size == 2;
+	S.has_word = P.score_size == 1 || P.score_size == 2;
+	if (e->pssm_n) {
+		S.bias = 0; S.max_mat = -128;
+		for (int32_t q = 0; q < e->n_q; ++q) { S.bias = std::max(S.bias, e->q_bias[q]); S.max_mat = std::max(S.max_mat, e->q_max[q]); }
+		S.limit_byte = 255 - S.bias;
+		S.limit_word = 32767 - std::max(S.max_mat, 0) - 256;
+		S.q_bias = e->q_bias.data(); S.q_max = e->q_max.data();
+		return e->upload_refs(P.n);
+	}
 	S.bias = 0; S.max_mat = -128;
 	for (int i = 0; i < P.n * P.n; ++i) { if (P.mat[i] < S.bias) S.bias = P.mat[i]; if (P.mat[i] > S.max_mat) S.max_mat = P.mat[i]; }
 	S.bias = S.bias < 0 ? -S.bias : S.bias;
 	S.limit_byte = 255 - S.bias;
 	S.limit_word = 32767 - std::max(S.max_mat, 0) - 256;
-	S.has_byte = P.score_size == 0 || P.score_size == 2;
-	S.has_word = P.score_size == 1 || P.score_size == 2;
 	if (e->d_mat.ensure((size_t)P.n * P.n + 16)) return -1;
 	SSW_CUDA_OK(cudaMemcpyAsync(e->d_mat.p, P.mat, (size_t)P.n * P.n, cudaMemcpyHostToDevice, e->stream));
 	return e->upload_refs(P.n);
@@ -2055,7 +2131,7 @@ static int engine_align_impl(ssw_engine* e, const ssw_batch_params* params,
                              ssw_batch_result* results,
                              uint32_t* cigar_pool, int64_t pool_cap, int64_t* pool_used)
 {
-	if (!e || !params || !params->mat || n_pairs < 0 || (n_pairs && !results)) return -1;
+	if (!scoring_args_ok(e, params, "ssw_engine_align") || n_pairs < 0 || (n_pairs && !results)) return -1;
 	if (n_pairs > 0 && (e->n_q <= 0 || e->n_r <= 0)) { fprintf(stderr, "[libssw-b200] ssw_engine_align: no resident sequences\n"); return -1; }
 	const ssw_batch_params& P = *params;
 	if (P.n < 1 || P.n > 64) { fprintf(stderr, "[libssw-b200] alphabet size %d not supported (1..64)\n", P.n); return -1; }
@@ -2132,6 +2208,7 @@ static int engine_align_impl(ssw_engine* e, const ssw_batch_params* params,
 				kid->n_q = e->n_q; kid->n_r = e->n_r; kid->q_off = e->q_off; kid->r_off = e->r_off; kid->r_len = e->r_len;
 				kid->padded_n = e->padded_n; kid->from_text = true;     /* no host copy: the padded references are the parent's */
 				kid->d_q.borrow(e->d_q); kid->d_r.borrow(e->d_r);
+				kid->pssm_n = e->pssm_n; kid->q_bias = e->q_bias; kid->q_max = e->q_max;
 				kid->opt = e->opt;
 			}
 			auto work = [&](int k) {
@@ -2363,7 +2440,7 @@ static int engine_search_impl(ssw_engine* e, const ssw_batch_params* params, int
                               int32_t* hit_ref, ssw_batch_result* hits, int32_t* n_hits,
                               uint32_t* cigar_pool, int64_t pool_cap, int64_t* pool_used)
 {
-	if (!e || !params || !params->mat) { fprintf(stderr, "[libssw-b200] ssw_engine_search: no engine or no parameters\n"); return -1; }
+	if (!scoring_args_ok(e, params, "ssw_engine_search")) return -1;
 	if (k < 1 || k > SSW_SEARCH_MAX_K) { fprintf(stderr, "[libssw-b200] ssw_engine_search: k = %d outside 1 .. %d\n", k, SSW_SEARCH_MAX_K); return -1; }
 	if (!hit_ref || !hits || !n_hits) { fprintf(stderr, "[libssw-b200] ssw_engine_search: NULL output array\n"); return -1; }
 	if (e->n_q <= 0 || e->n_r <= 0) { fprintf(stderr, "[libssw-b200] ssw_engine_search: no resident sequences\n"); return -1; }
@@ -2407,7 +2484,7 @@ static int engine_search_all_impl(ssw_engine* e, const ssw_batch_params* params,
 {
 	if (!out) { fprintf(stderr, "[libssw-b200] ssw_engine_search_all: NULL output\n"); return -1; }
 	*out = nullptr;
-	if (!e || !params || !params->mat) { fprintf(stderr, "[libssw-b200] ssw_engine_search_all: no engine or no parameters\n"); return -1; }
+	if (!scoring_args_ok(e, params, "ssw_engine_search_all")) return -1;
 	if (max_hits < 0) { fprintf(stderr, "[libssw-b200] ssw_engine_search_all: max_hits = %lld is negative\n", (long long)max_hits); return -1; }
 	if (e->n_q <= 0 || e->n_r <= 0) { fprintf(stderr, "[libssw-b200] ssw_engine_search_all: no resident sequences\n"); return -1; }
 	const ssw_batch_params& P = *params;
@@ -2463,6 +2540,7 @@ static int mark_mismatch_impl(ssw_engine* e, int64_t n_pairs, const int32_t* pai
 	if (!e || n_pairs < 0 || (n_pairs && !results) || !out_used) return -1;
 	if ((pair_query == nullptr) != (pair_ref == nullptr)) return -1;
 	*out_used = 0;
+	if (e->pssm_n) { fprintf(stderr, "[libssw-b200] ssw_engine_mark_mismatch: query profiles are resident: there are no query letters to compare\n"); return -1; }
 	if (n_pairs > 0 && (e->n_q <= 0 || e->n_r <= 0)) return -1;
 	SSW_CUDA_OK(cudaSetDevice(e->device));
 	std::vector<SswMarkTask> tasks;

@@ -110,14 +110,47 @@ static inline size_t ssw_fill_smem_bytes(int n, int warps = SSW_FILL_WARPS) { re
 /* shared device code                                                                                          */
 /* ---------------------------------------------------------------------------------------------------------- */
 
+/* The profile rows of ssw_build_profile from position-specific query profiles (ssw_engine_set_sequences_pssm): `pssm` holds n
+ * scores per row, SswQuery.off counts rows, real row r scores pssm[(off + r) * n + letter]; only rows < len are read.  A row is
+ * addressed as a 32-bit offset r * n from its query's first row (the host bounds len * n), as codes are in the matrix. */
+template <int R>
+__device__ static __forceinline__ void ssw_build_profile_pssm(uint32_t* prof, int lane, int row0, const SswQuery& qa, const SswQuery& qb,
+                                                             const int8_t* __restrict__ pssm, int n, int letter0, int letter_step)
+{
+	const int8_t* pa = pssm + (int64_t)qa.off * n;
+	const int8_t* pb = pssm + (int64_t)qb.off * n;
+	int ca[R], cb[R];
+#pragma unroll
+	for (int k = 0; k < R; ++k) {
+		const int row = row0 + k;
+		ca[k] = row < qa.len ? (qa.rev ? qa.len - 1 - row : row) * n : (row < qa.lp ? -1 : -2);
+		cb[k] = row < qb.len ? (qb.rev ? qb.len - 1 - row : row) * n : (row < qb.lp ? -1 : -2);
+	}
+	for (int letter = letter0; letter <= n; letter += letter_step) {
+		uint32_t* pl = prof + letter * (32 * SswProfRows<R>::S);
+#pragma unroll
+		for (int k = 0; k < R; ++k) {
+			int a = SSW_NEG16, b = SSW_NEG16;
+			if (letter < n) {
+				a = ca[k] >= 0 ? (int)pa[ca[k] + letter] : (ca[k] == -1 ? 0 : SSW_NEG16);
+				b = cb[k] >= 0 ? (int)pb[cb[k] + letter] : (cb[k] == -1 ? 0 : SSW_NEG16);
+			}
+			pl[ssw_prof_slot<R>(k, lane)] = pack2(a, b);
+		}
+	}
+}
+
 /* Build the packed profile rows [row0, row0 + R) of this lane for both queries into `prof`
  * (qP_byte / qP_word analogue, ssw.c:163-188 / :388-410): real rows score mat[letter][code], pad rows 0,
- * rows beyond the query's padded length and the null letter n score -32768 (dead: H stays 0). */
-template <int R>
+ * rows beyond the query's padded length and the null letter n score -32768 (dead: H stays 0).
+ * PSSM: the queries are position-specific profiles (ssw_build_profile_pssm; the host passes mat == nullptr).  A template
+ * parameter of the kernels, so that their instances for query codes are compiled from the same code as without profiles. */
+template <int R, bool PSSM = false>
 __device__ static __forceinline__ void ssw_build_profile(uint32_t* prof, int lane, int row0, const SswQuery& qa, const SswQuery& qb,
                                                         const int8_t* __restrict__ qcodes, const int8_t* __restrict__ mat, int n,
                                                         int letter0 = 0, int letter_step = 1)
 {
+	if constexpr (PSSM) { ssw_build_profile_pssm<R>(prof, lane, row0, qa, qb, qcodes, n, letter0, letter_step); return; }
 	int ca[R], cb[R];
 #pragma unroll
 	for (int k = 0; k < R; ++k) {
@@ -378,7 +411,7 @@ __device__ static __forceinline__ void ssw_reduce_best(const SswLaneBest& lb, in
  * lane) that four-warp CTAs would leave the SM with 8 resident warps -- eight warps per profile keep 16. */
 /* ARM: items may carry a late arming position (SswItem.cend, device-planned grids); a template parameter so that the kernels
  * that never use it do not pay for the extra predicate per step. */
-template <int G, int R, int DIR, int CM, bool TERM, int WARPS = SSW_FILL_WARPS, bool ARM = false>
+template <int G, int R, int DIR, int CM, bool TERM, int WARPS = SSW_FILL_WARPS, bool ARM = false, bool PSSM = false>
 __global__ void __launch_bounds__(WARPS * 32, WARPS == SSW_FILL_WARPS ? SSW_FILL_MINB : 2)
 ssw_fill_kernel(const SswItem* __restrict__ items, int n_items,
                 const int8_t* __restrict__ qcodes, const int8_t* __restrict__ refs,
@@ -412,10 +445,10 @@ ssw_fill_kernel(const SswItem* __restrict__ items, int n_items,
 
 	if (share) {
 		const SswItem& first = items[(int)blockIdx.x * nwarps * GPW];               /* always a live item */
-		ssw_build_profile<R>(prof, lane, t * R, first.qa, first.qb, qcodes, mat, n, warp, nwarps);
+		ssw_build_profile<R, PSSM>(prof, lane, t * R, first.qa, first.qb, qcodes, mat, n, warp, nwarps);
 		__syncthreads();
 	} else {
-		ssw_build_profile<R>(prof, lane, t * R, it.qa, it.qb, qcodes, mat, n);
+		ssw_build_profile<R, PSSM>(prof, lane, t * R, it.qa, it.qb, qcodes, mat, n);
 		__syncwarp();
 	}
 
@@ -681,7 +714,7 @@ __device__ static __forceinline__ void ssw_st_release(volatile int* p, int v)
 }
 #endif
 
-template <int R, int DIR, bool TERM, bool SPLIT>
+template <int R, int DIR, bool TERM, bool SPLIT, bool PSSM = false>
 __global__ void __launch_bounds__(SSW_STRIP_MAXW * 32)
 ssw_fill_strips_kernel(const SswStripTask* __restrict__ tasks,
                        const int8_t* __restrict__ qcodes, const int8_t* __restrict__ refs,
@@ -741,7 +774,7 @@ ssw_fill_strips_kernel(const SswStripTask* __restrict__ tasks,
 			if (hi <= lo) continue;
 			if (TERM) { int st = lane == 0 ? *stop : 0; st = __shfl_sync(FULL, st, 0); if (st) break; }
 
-			ssw_build_profile<R>(prof, lane, s * 32 * R + lane * R, T.qa, T.qb, qcodes, mat, n);
+			ssw_build_profile<R, PSSM>(prof, lane, s * 32 * R + lane * R, T.qa, T.qb, qcodes, mat, n);
 			__syncwarp();
 
 			/* lane registers: fresh at the strip's first column, else un-parked */

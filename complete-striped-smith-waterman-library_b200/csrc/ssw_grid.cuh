@@ -17,13 +17,15 @@
 #include "ssw_common.cuh"
 #include "../../include/ssw_batch.h"
 
-struct SswGridQ { int32_t off, len, lp, mask_len; };      /* one query: slice, padded rows of this pass, mask window */
+/* one query: slice, padded rows of this pass, mask window, the score limit of this pass (SswAlnDesc.limit: per query, as query
+ * profiles have their own byte bias) */
+struct SswGridQ { int32_t off, len, lp, mask_len, limit; };
 
 struct SswGridArgs {
 	int32_t n_qp;        /* query pairs in this launch */
 	int32_t n_r;         /* references */
 	int32_t n_r_pad;     /* references rounded up to a whole number of CTAs (dead items in between) */
-	int32_t word, limit;
+	int32_t word;
 	int32_t arm_tail;    /* > 0: best-cell rows are recorded in the last arm_tail columns of every reference only (SswItem.cend) */
 	int64_t cm_words_per_qp;
 };
@@ -48,7 +50,7 @@ ssw_grid_plan_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGridQ*
 	it.qa.off = qa.off; it.qa.len = qa.len; it.qa.lp = qa.lp; it.qa.rev = 0;
 	it.qb.off = 0; it.qb.len = 0; it.qb.lp = 0; it.qb.rev = 0;
 	SswGridQ qb;
-	qb.off = 0; qb.len = 0; qb.lp = 0; qb.mask_len = 0;
+	qb.off = 0; qb.len = 0; qb.lp = 0; qb.mask_len = 0; qb.limit = 0;
 	if (pr.y >= 0) { qb = qt[pr.y]; it.qb.off = qb.off; it.qb.len = qb.len; it.qb.lp = qb.lp; }
 	it.ref_off = ref_off[r]; it.ref_len = ref_len[r];
 	it.cend = (A.arm_tail > 0 && live) ? max(0, ref_len[r] - A.arm_tail) : 0;
@@ -58,10 +60,10 @@ ssw_grid_plan_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGridQ*
 	if (live) {
 		SswAlnDesc d;
 		d.first_item = (int32_t)idx; d.n_items = 1; d.half = 0; d.ref_len = it.ref_len; d.read_len = qa.len;
-		d.word = A.word; d.limit = A.limit; d.mask_len = qa.mask_len; d.cm_off = it.cm_off; d.scan_all = 0; d.warm = 0; d.byte_pad = 0;
+		d.word = A.word; d.limit = qa.limit; d.mask_len = qa.mask_len; d.cm_off = it.cm_off; d.scan_all = 0; d.warm = 0; d.byte_pad = 0;
 		const int64_t di = ((int64_t)pi * A.n_r + r) * 2;
 		descs[di] = d;
-		d.half = 1; d.read_len = qb.len; d.mask_len = qb.mask_len;
+		d.half = 1; d.read_len = qb.len; d.mask_len = qb.mask_len; d.limit = qb.limit;
 		if (pr.y < 0) d.n_items = 0;                                   /* no second query: the resolve kernel skips it */
 		descs[di + 1] = d;
 	}

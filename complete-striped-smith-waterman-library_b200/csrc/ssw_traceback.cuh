@@ -49,7 +49,7 @@ enum { SSW_TB_OK = 0, SSW_TB_WIDER = 1, SSW_TB_ERROR = 2, SSW_TB_MISMATCH = 3 };
 
 struct SswTbTask {
 	int64_t ref_off;     /* offset of ref[ref_begin1] in the padded reference array */
-	int64_t read_off;    /* offset of read[read_begin1] in the query array */
+	int64_t read_off;    /* offset of read[read_begin1] in the query array (query profiles: of its row's first byte) */
 	int32_t ref_len, read_len, score;
 	int32_t bw;          /* band half-width of this round */
 	int32_t max, max_i, max_j;   /* running maximum carried across band doublings */
@@ -74,8 +74,20 @@ __device__ static __forceinline__ int64_t ssw_globaltimer()
 }
 __device__ static __forceinline__ uint32_t ssw_tb_pack(uint32_t len, uint32_t op) { return (len << 4) | op; }  /* op: M0 I1 D2 */
 
+/* PSSM: the queries are position-specific profiles (ssw_engine_set_sequences_pssm), `read` points at the task's first profile row
+ * (n scores per row) and there is no matrix.  rd stands for read row i: its code (smat[letter * n + code]) or, with profiles,
+ * its byte offset i * n (read[i * n + letter]). */
+template <bool PSSM>
+__device__ static __forceinline__ int ssw_tb_rd(const int8_t* read, int n, int i) { return PSSM ? i * n : (int)read[i]; }
+template <bool PSSM>
+__device__ static __forceinline__ int ssw_tb_score(const int8_t* smat, const int8_t* read, int n, int letter, int rd)
+{
+	return PSSM ? (int)read[rd + letter] : (int)smat[letter * n + rd];
+}
+
 /* Decide whether the band must be doubled (ssw.c:678-679); if not, walk the traceback (ssw.c:683-762) from the
  * maximum cell, run-length encode it and re-score the CIGAR (ssw.c:785-811).  One thread. */
+template <bool PSSM>
 __device__ static void ssw_tb_finish(SswTbTask& T, SswTbTask* slot, const int8_t* ref, const int8_t* read,
                                      const int8_t* __restrict__ mat, int n, int gapO, int gapE,
                                      const uint8_t* dir, uint32_t* cig_base)
@@ -116,7 +128,7 @@ __device__ static void ssw_tb_finish(SswTbTask& T, SswTbTask* slot, const int8_t
 	for (int k = 0; k < l; ++k) {
 		const uint32_t clen = cig[k] >> 4, cop = cig[k] & 15;
 		if (cop == 0) {
-			for (uint32_t x = 0; x < clen; ++x) { sc += (int)mat[(int)ref[rp] * n + (int)read[qp]]; ++rp; ++qp; }
+			for (uint32_t x = 0; x < clen; ++x) { sc += ssw_tb_score<PSSM>(mat, read, n, (int)ref[rp], ssw_tb_rd<PSSM>(read, n, qp)); ++rp; ++qp; }
 		} else {
 			sc -= gapO + (clen > 1 ? (int)(clen - 1) * gapE : 0);
 			if (cop == 1) qp += (int)clen; else rp += (int)clen;
@@ -237,10 +249,10 @@ __device__ static __forceinline__ void ssw_tb_tiles(const bool (&act)[NT], int i
 }
 
 /* one group of NT tiles of row i starting at column j0: loads from the row ring, ssw_tb_tiles, stores */
-template <int NT, bool LAST, bool PRE = false>
+template <bool PSSM, int NT, bool LAST, bool PRE = false>
 __device__ static __forceinline__ void ssw_tb_row_group(int i, int j0, int beg, int end, int pbeg, bool top_oob, int lane, int rd,
                                                        const int32_t* Hprev, const int32_t* Eprev, int32_t* Hcur, int32_t* Ecur, int mask,
-                                                       const int8_t* smat, int n, const int8_t* ref, uint8_t* drow,
+                                                       const int8_t* smat, const int8_t* read, int n, const int8_t* ref, uint8_t* drow,
                                                        int gapO, int gapE, int g, int& carryF, int& carryFp,
                                                        int& bestv, int& besti, int& bestj, const int* spre = nullptr)
 {
@@ -256,7 +268,7 @@ __device__ static __forceinline__ void ssw_tb_row_group(int i, int j0, int beg, 
 				if (!(j[t] == end && top_oob)) { Hup[t] = Hprev[j[t] & mask]; Eup[t] = Eprev[j[t] & mask]; }
 				if (j[t] - 1 >= pbeg) Hdg[t] = Hprev[(j[t] - 1) & mask];
 			}
-			s[t] = PRE ? spre[t] : (int)smat[(int)ref[j[t]] * n + rd];      /* PRE: looked up ahead of the row (first group) */
+			s[t] = PRE ? spre[t] : ssw_tb_score<PSSM>(smat, read, n, (int)ref[j[t]], rd);      /* PRE: looked up ahead of the row (first group) */
 		}
 	}
 	ssw_tb_tiles<NT, LAST>(act, i, j, beg, lane, Hup, Eup, Hdg, s, gapO, gapE, g, carryF, carryFp, Hv, Ev, dirb,
@@ -283,6 +295,7 @@ __host__ __device__ static __forceinline__ int ssw_tb_ring_of(int bw)
 
 /* One banded fill (ssw.c:628-676) by one warp: rows in the warp's shared-memory ring `mine` (4 x ring ints), direction bytes
  * to `dir`, returns the first row-major cell holding the maximum of this band (all lanes). */
+template <bool PSSM>
 __device__ static __forceinline__ void ssw_tb_band_fill(int lane, int ql, int rl, int bw, const int8_t* ref, const int8_t* read,
                                                        const int8_t* smat, int n, int gapO, int gapE, int g,
                                                        int32_t* mine, int ring, uint8_t* dir, int& bestv, int& besti, int& bestj)
@@ -291,7 +304,7 @@ __device__ static __forceinline__ void ssw_tb_band_fill(int lane, int ql, int rl
 	const int mask = ring - 1;
 	const int W = 2 * bw + 1;
 	bestv = 0; besti = 0; bestj = 0;
-	int rd_next = (int)read[0];
+	int rd_next = ssw_tb_rd<PSSM>(read, n, 0);
 	int letn[4];                                         /* reference letters of the next row's first group (clamped into the reference) */
 #pragma unroll
 	for (int t = 0; t < 4; ++t) letn[t] = (int)ref[min(32 * t + lane, rl - 1)];
@@ -307,14 +320,14 @@ __device__ static __forceinline__ void ssw_tb_band_fill(int lane, int ql, int rl
 		const int pbeg = max(0, i - 1 - bw);
 		const bool top_oob = (i <= bw + 1) || (end == i + bw);
 		const int rd = rd_next;
-		if (i + 1 < ql) rd_next = (int)read[i + 1];
+		if (i + 1 < ql) rd_next = ssw_tb_rd<PSSM>(read, n, i + 1);
 		uint8_t* drow = dir + (size_t)W * i - beg;
 		/* scores of the row's first group from the letters fetched during the previous row (the letter fetch and the matrix
 		 * look-up behind it would otherwise head the row's dependent chain), then the letters of the next row's first group */
 		int spre[4];
 #if SSW_TB_PRE
 #pragma unroll
-		for (int t = 0; t < 4; ++t) spre[t] = (int)smat[letn[t] * n + rd];
+		for (int t = 0; t < 4; ++t) spre[t] = ssw_tb_score<PSSM>(smat, read, n, letn[t], rd);
 		{
 			const int begn = max(0, i + 1 - bw);
 #pragma unroll
@@ -325,7 +338,7 @@ __device__ static __forceinline__ void ssw_tb_band_fill(int lane, int ql, int rl
 			int carryF = -gapO, carryFp = 0;
 			int j0 = beg;
 #define SSW_TB_GROUP(NT, LAST, PRE)                                                                                          \
-			ssw_tb_row_group<NT, LAST, PRE>(i, j0, beg, end, pbeg, top_oob, lane, rd, Hp, Ep, Hc, Ec, mask, smat, n, ref, drow,      \
+			ssw_tb_row_group<PSSM, NT, LAST, PRE>(i, j0, beg, end, pbeg, top_oob, lane, rd, Hp, Ep, Hc, Ec, mask, smat, read, n, ref, drow, \
 			                                gapO, gapE, g, carryF, carryFp, bestv, besti, bestj, spre)
 			if (j0 <= end) {                                  /* first group: scores looked up ahead */
 				const int tiles = (end - j0) / 32 + 1;
@@ -355,6 +368,7 @@ __device__ static __forceinline__ void ssw_tb_band_fill(int lane, int ql, int rl
 /* Traceback (ssw.c:683-762) of the finished band T.bw by one warp, staged through `stage` (shared memory, stage_bytes): the warp
  * copies blocks of direction bytes with coalesced loads and lane 0 walks inside them (the plain walk pays a DRAM latency per
  * step because every step moves up one band row); then the CIGAR re-scoring (ssw.c:785-811).  Writes the task record. */
+template <bool PSSM>
 __device__ static __forceinline__ void ssw_tb_walk(SswTbTask& T, SswTbTask* slot, int lane, const uint8_t* dir, uint8_t* stage, int stage_bytes,
                                                   uint32_t* cig, const int8_t* smat, const int8_t* ref, const int8_t* read, int n,
                                                   int gapO, int gapE, long long c1)
@@ -421,7 +435,7 @@ __device__ static __forceinline__ void ssw_tb_walk(SswTbTask& T, SswTbTask* slot
 	for (int k = 0; k < l; ++k) {
 		const uint32_t clen = cig[k] >> 4, cop = cig[k] & 15;
 		if (cop == 0) {
-			for (uint32_t x = 0; x < clen; ++x) { sc += (int)smat[(int)ref[rp] * n + (int)read[qp]]; ++rp; ++qp; }
+			for (uint32_t x = 0; x < clen; ++x) { sc += ssw_tb_score<PSSM>(smat, read, n, (int)ref[rp], ssw_tb_rd<PSSM>(read, n, qp)); ++rp; ++qp; }
 		} else {
 			sc -= gapO + (clen > 1 ? (int)(clen - 1) * gapE : 0);
 			if (cop == 1) qp += (int)clen; else rp += (int)clen;
@@ -441,6 +455,7 @@ __device__ static __forceinline__ void ssw_tb_walk(SswTbTask& T, SswTbTask* slot
  */
 #define SSW_TBP_MAXBW 990
 
+template <bool PSSM>
 __global__ void __launch_bounds__(SSW_TB_THREADS)
 ssw_banded_smem_kernel(SswTbTask* __restrict__ tasks, int n_tasks,
                        const int8_t* __restrict__ qcodes, const int8_t* __restrict__ refs,
@@ -450,7 +465,7 @@ ssw_banded_smem_kernel(SswTbTask* __restrict__ tasks, int n_tasks,
 	SSW_DYN_SMEM(int32_t, smem);                                  /* [warp][4][ring] ints, then n*n matrix bytes */
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	int8_t* smat = reinterpret_cast<int8_t*>(smem + (size_t)SSW_TB_WARPS * 4 * ring);
-	for (int k = threadIdx.x; k < n * n; k += blockDim.x) smat[k] = mat[k];
+	if (!PSSM) for (int k = threadIdx.x; k < n * n; k += blockDim.x) smat[k] = mat[k];
 	__syncthreads();
 	const int ti = (int)blockIdx.x * SSW_TB_WARPS + warp;
 	if (ti >= n_tasks) return;
@@ -470,7 +485,7 @@ ssw_banded_smem_kernel(SswTbTask* __restrict__ tasks, int n_tasks,
 	 * row ring: only the last band's directions are needed, and the running maximum is carried in T */
 	for (;;) {
 		int bestv, besti, bestj;
-		ssw_tb_band_fill(lane, ql, rl, bw, ref, read, smat, n, gapO, gapE, g, mine, ring, dir, bestv, besti, bestj);
+		ssw_tb_band_fill<PSSM>(lane, ql, rl, bw, ref, read, smat, n, gapO, gapE, g, mine, ring, dir, bestv, besti, bestj);
 		if (bestv > T.max) { T.max = bestv; T.max_i = besti; T.max_j = bestj; }     /* strict, carried across doublings */
 		if (!(T.max < T.score && 2 * bw <= len)) break;                              /* ssw.c:678-679: done */
 		if (2 * (2 * bw) + 66 > ring) {                                              /* the next band needs a wider ring: back to the host */
@@ -486,7 +501,7 @@ ssw_banded_smem_kernel(SswTbTask* __restrict__ tasks, int n_tasks,
 	T.dbg_fill = c1 - c0; T.dbg_walk = 0; T.dbg_score = 0;
 	__threadfence_block();
 	__syncwarp();
-	ssw_tb_walk(T, tasks + ti, lane, dir, reinterpret_cast<uint8_t*>(mine), 4 * ring * (int)sizeof(int32_t), cig_base + T.cig_off,
+	ssw_tb_walk<PSSM>(T, tasks + ti, lane, dir, reinterpret_cast<uint8_t*>(mine), 4 * ring * (int)sizeof(int32_t), cig_base + T.cig_off,
 	            smat, ref, read, n, gapO, gapE, c1);
 }
 
@@ -505,7 +520,7 @@ ssw_banded_smem_kernel(SswTbTask* __restrict__ tasks, int n_tasks,
 #define SSW_TBS_MAXW 8
 __host__ __device__ static __forceinline__ size_t ssw_tb_dir_bytes(int bw, int read_len) { return (((size_t)(2 * bw + 1) * (size_t)read_len + 2) + 15) / 16 * 16; }
 
-template <int DUMMY = 0>
+template <bool PSSM>
 __global__ void __launch_bounds__(SSW_TBS_MAXW * 32)
 ssw_banded_spec_kernel(SswTbTask* __restrict__ tasks, int n_tasks,
                        const int8_t* __restrict__ qcodes, const int8_t* __restrict__ refs,
@@ -517,7 +532,7 @@ ssw_banded_spec_kernel(SswTbTask* __restrict__ tasks, int n_tasks,
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const int mat_ints = (n * n + 15) / 16 * 4;
 	int8_t* smat = reinterpret_cast<int8_t*>(smem);
-	for (int k = threadIdx.x; k < n * n; k += blockDim.x) smat[k] = mat[k];
+	if (!PSSM) for (int k = threadIdx.x; k < n * n; k += blockDim.x) smat[k] = mat[k];
 	__syncthreads();
 	const int ti = (int)blockIdx.x;
 	if (ti >= n_tasks) return;
@@ -546,7 +561,7 @@ ssw_banded_spec_kernel(SswTbTask* __restrict__ tasks, int n_tasks,
 	uint8_t* dir = dir_base + T.dir_off + dir_off + 1;
 	if (warp < nw && possible) {
 		int bestv, besti, bestj;
-		ssw_tb_band_fill(lane, ql, rl, bw, ref, read, smat, n, gapO, gapE, g, smem + ring_off, ssw_tb_ring_of(bw), dir, bestv, besti, bestj);
+		ssw_tb_band_fill<PSSM>(lane, ql, rl, bw, ref, read, smat, n, gapO, gapE, g, smem + ring_off, ssw_tb_ring_of(bw), dir, bestv, besti, bestj);
 		if (lane == 0) { s_best[warp][0] = bestv; s_best[warp][1] = besti; s_best[warp][2] = bestj; }
 	}
 	__threadfence_block();
@@ -569,11 +584,12 @@ ssw_banded_spec_kernel(SswTbTask* __restrict__ tasks, int n_tasks,
 		if (lane == 0) { T.status = SSW_TB_WIDER; tasks[ti] = T; }
 		return;
 	}
-	ssw_tb_walk(T, tasks + ti, lane, dir_base + T.dir_off + done_off + 1, reinterpret_cast<uint8_t*>(smem + mat_ints),
+	ssw_tb_walk<PSSM>(T, tasks + ti, lane, dir_base + T.dir_off + done_off + 1, reinterpret_cast<uint8_t*>(smem + mat_ints),
 	            (total_ints - mat_ints) * (int)sizeof(int32_t), cig_base + T.cig_off, smat, ref, read, n, gapO, gapE, c1);
 }
 
 /* General variant (any band width): one warp per alignment, H/E rows in global memory. */
+template <bool PSSM>
 __global__ void __launch_bounds__(SSW_TB_THREADS)
 ssw_banded_kernel(SswTbTask* __restrict__ tasks, int n_tasks,
                   const int8_t* __restrict__ qcodes, const int8_t* __restrict__ refs,
@@ -601,7 +617,7 @@ ssw_banded_kernel(SswTbTask* __restrict__ tasks, int n_tasks,
 		const int beg = max(0, i - bw), end = min(rl - 1, i + bw);
 		const int pbeg = max(0, i - 1 - bw);
 		const bool top_oob = (i <= bw + 1) || (end == i + bw);   /* cell above column `end` reads as outside the band */
-		const int rd = (int)read[i];
+		const int rd = ssw_tb_rd<PSSM>(read, n, i);
 		uint8_t* drow = dir + (size_t)W * i - beg;              /* drow[j] is the cell of column j */
 		int carryF = -gapO;                                      /* F of the tile's first column; F(beg) = max(0-gapO, neg_inf-gapE) */
 		int carryH = 0, carryFp = 0;                             /* H, F of the column left of the tile */
@@ -614,7 +630,7 @@ ssw_banded_kernel(SswTbTask* __restrict__ tasks, int n_tasks,
 					if (!(j == end && top_oob)) { Hup = Hrow[prv][j]; Eup = Erow[prv][j]; }
 					if (j - 1 >= pbeg) Hdg = Hrow[prv][j - 1];
 				}
-				s = (int)mat[(int)ref[j] * n + rd];
+				s = ssw_tb_score<PSSM>(mat, read, n, (int)ref[j], rd);
 			}
 			int Hv, Ev, dirb;
 			ssw_tb_tile(act, i, j, beg, lane, Hup, Eup, Hdg, s, gapO, gapE, g, carryF, carryH, carryFp, Hv, Ev, dirb);
@@ -636,7 +652,7 @@ ssw_banded_kernel(SswTbTask* __restrict__ tasks, int n_tasks,
 	if (bestv > T.max) { T.max = bestv; T.max_i = besti; T.max_j = bestj; }     /* strict, carried across doublings */
 	__threadfence_block();
 	__syncwarp();
-	if (lane == 0) ssw_tb_finish(T, tasks + ti, ref, read, mat, n, gapO, gapE, dir, cig_base);
+	if (lane == 0) ssw_tb_finish<PSSM>(T, tasks + ti, ref, read, mat, n, gapO, gapE, dir, cig_base);
 }
 
 /*
@@ -661,7 +677,8 @@ ssw_cigar_pack_kernel(const SswTbTask* __restrict__ tasks, int n_tasks, const ui
 
 static int ssw_traceback_run(cudaStream_t stream, cudaStream_t* side /* 3 side streams of the caller, created on demand */,
                              std::vector<SswTbTask>& tasks,
-                             const int8_t* d_q, const int8_t* d_r, const int8_t* d_mat, int n, int gapO, int gapE,
+                             const int8_t* d_q, const int8_t* d_r,
+                             const int8_t* d_mat /* nullptr: d_q holds query profiles and read_off counts their bytes */, int n, int gapO, int gapE,
                              SswDevBuf* scratch, float* ms_acc, int64_t* launches,
                              int tb_maxbw /* "tb_maxbw" option: bands above this use the global-memory kernel (tests: 0) */,
                              bool carve /* "carve" option: largest shared-memory carve-out for the traceback kernels */,
@@ -775,16 +792,18 @@ static int ssw_traceback_run(cudaStream_t stream, cudaStream_t* side /* 3 side s
 					for (int w = 0; w < nw; ++w) { ints += 4 * (size_t)ssw_tb_ring_of(b2); b2 *= 2; }
 					smem = std::max(smem, ints * sizeof(int32_t));
 				}
-				if (ssw_ensure_dyn_smem(reinterpret_cast<const void*>(ssw_banded_spec_kernel<0>), smem)) return -1;
-				if (carve && ssw_prefer_max_smem(reinterpret_cast<const void*>(ssw_banded_spec_kernel<0>))) return -1;
-				ssw_launch(ssw_banded_spec_kernel<0>, dim3((unsigned)cnt), dim3(nw * 32), smem, st, d_tasks + g0, cnt, d_q, d_r, d_mat, n, gapO, gapE, base, d_cig, nw);
+				auto kern = d_mat ? ssw_banded_spec_kernel<false> : ssw_banded_spec_kernel<true>;
+				if (ssw_ensure_dyn_smem(reinterpret_cast<const void*>(kern), smem)) return -1;
+				if (carve && ssw_prefer_max_smem(reinterpret_cast<const void*>(kern))) return -1;
+				ssw_launch(kern, dim3((unsigned)cnt), dim3(nw * 32), smem, st, d_tasks + g0, cnt, d_q, d_r, d_mat, n, gapO, gapE, base, d_cig, nw);
 			} else if (ring) {
 				const size_t smem = (size_t)SSW_TB_WARPS * 4 * (size_t)ring * sizeof(int32_t) + (size_t)n * n + 16;
-				if (ssw_ensure_dyn_smem(reinterpret_cast<const void*>(ssw_banded_smem_kernel), smem)) return -1;
-				if (carve && ssw_prefer_max_smem(reinterpret_cast<const void*>(ssw_banded_smem_kernel))) return -1;
-				ssw_launch(ssw_banded_smem_kernel, grid, dim3(SSW_TB_THREADS), smem, st, d_tasks + g0, cnt, d_q, d_r, d_mat, n, gapO, gapE, base, d_cig, ring);
+				auto kern = d_mat ? ssw_banded_smem_kernel<false> : ssw_banded_smem_kernel<true>;
+				if (ssw_ensure_dyn_smem(reinterpret_cast<const void*>(kern), smem)) return -1;
+				if (carve && ssw_prefer_max_smem(reinterpret_cast<const void*>(kern))) return -1;
+				ssw_launch(kern, grid, dim3(SSW_TB_THREADS), smem, st, d_tasks + g0, cnt, d_q, d_r, d_mat, n, gapO, gapE, base, d_cig, ring);
 			} else {
-				ssw_launch(ssw_banded_kernel, grid, dim3(SSW_TB_THREADS), 0, st, d_tasks + g0, cnt, d_q, d_r, d_mat, n, gapO, gapE,
+				ssw_launch(d_mat ? ssw_banded_kernel<false> : ssw_banded_kernel<true>, grid, dim3(SSW_TB_THREADS), 0, st, d_tasks + g0, cnt, d_q, d_r, d_mat, n, gapO, gapE,
 				           base, reinterpret_cast<int32_t*>(base + off_rows), d_cig);
 			}
 			SSW_CUDA_OK(cudaGetLastError());

@@ -130,6 +130,11 @@ def _i8(a):
     return a, a.ctypes.data_as(ct.POINTER(ct.c_int8))
 
 
+def _mat(mat):
+    """(array kept alive, pointer) of a scoring matrix; None -> NULL (query profiles resident)."""
+    return (None, None) if mat is None else _i8(mat)
+
+
 def concat(seqs):
     """List of int8 code arrays -> (concatenation, int64 offsets[n+1])."""
     off = np.zeros(len(seqs) + 1, dtype=np.int64)
@@ -201,6 +206,27 @@ class BatchAligner(object):
         self.n_q, self.n_r = len(queries), len(refs)
         self._lens = (np.diff(qo), np.diff(ro))
 
+    def set_profiles(self, profiles, refs, n):
+        """Host -> device copy of query profiles (PSSMs) and references (ssw_engine_set_sequences_pssm): `profiles` is a list of
+        (L_q, n) int8 arrays, row i = the scores of query position i against the n reference letters; `refs` int8 code arrays.
+        Later align / search / search_all calls take mat=None and this n."""
+        rows = [np.asarray(p, dtype=np.int8).reshape(-1, n) if n > 0 else np.asarray(p, dtype=np.int8) for p in profiles]
+        qo = np.zeros(len(rows) + 1, dtype=np.int64)
+        if rows:
+            qo[1:] = np.cumsum([len(p) for p in rows])
+        qc = np.ascontiguousarray(np.concatenate([p.reshape(-1) for p in rows]) if rows else np.zeros(0, np.int8))
+        rc, ro = concat(refs)
+        f = self.lib.ssw_engine_set_sequences_pssm
+        f.argtypes = [ct.c_void_p, ct.c_int32, ct.POINTER(ct.c_int8), ct.POINTER(ct.c_int64), ct.c_int32,
+                      ct.c_int32, ct.POINTER(ct.c_int8), ct.POINTER(ct.c_int64)]
+        f.restype = ct.c_int
+        rv = f(self.h, len(rows), qc.ctypes.data_as(ct.POINTER(ct.c_int8)), qo.ctypes.data_as(ct.POINTER(ct.c_int64)), int(n),
+               len(refs), rc.ctypes.data_as(ct.POINTER(ct.c_int8)), ro.ctypes.data_as(ct.POINTER(ct.c_int64)))
+        if rv:
+            raise RuntimeError("ssw_engine_set_sequences_pssm failed (%d)" % rv)
+        self.n_q, self.n_r = len(rows), len(refs)
+        self._lens = (np.diff(qo), np.diff(ro))
+
     def set_sequences_text(self, queries, refs, table, n, add_reverse_complement=False):
         """Sequences as text (bytes / str): translated to codes with `table` (128 int8 entries) on the device; with
         add_reverse_complement the reverse complement of query k becomes query len(queries) + k."""
@@ -251,10 +277,11 @@ class BatchAligner(object):
 
     def align(self, mat, n, gap_open=3, gap_extend=1, flag=0, filters=0, filterd=0, mask_len=-1, score_size=2,
               pair_query=None, pair_ref=None, want_cigar=None, out=None):
-        """Align pairs of the resident sequences; returns (results[RESULT_DTYPE], cigar_pool[uint32]).
+        """Align pairs of the resident sequences; returns (results[RESULT_DTYPE], cigar_pool[uint32]).  mat=None with query
+        profiles resident (set_profiles).
         out: a results array of a previous call with the same number of pairs to write into (large grids return
         hundreds of MB of records; re-using the buffer avoids mapping and unmapping it on every call)."""
-        mat, matp = _i8(mat)
+        mat, matp = _mat(mat)
         P = BatchParams(matp, n, gap_open, gap_extend, flag, filters, filterd, mask_len, score_size)
         if pair_query is None:
             n_pairs = self.n_q * self.n_r
@@ -289,12 +316,12 @@ class BatchAligner(object):
         """Top-k search of every resident query against all resident references (ssw_engine_search).  Returns
         (hit_ref[n_q, k] int32, hits[n_q, k] RESULT_DTYPE, n_hits[n_q] int32, cigar_pool[uint32]): row q holds query q's
         n_hits[q] best hits in rank order (status-1 pairs, then score1 descending, then reference ascending); unused slots
-        have hit_ref -1."""
+        have hit_ref -1.  mat=None with query profiles resident."""
         f = self.lib.ssw_engine_search
         f.argtypes = [ct.c_void_p, ct.POINTER(BatchParams), ct.c_int32, ct.c_int32, ct.POINTER(ct.c_int32), ct.c_void_p,
                       ct.POINTER(ct.c_int32), ct.POINTER(ct.c_uint32), ct.c_int64, ct.POINTER(ct.c_int64)]
         f.restype = ct.c_int
-        mat, matp = _i8(mat)
+        mat, matp = _mat(mat)
         P = BatchParams(matp, n, gap_open, gap_extend, flag, filters, filterd, mask_len, score_size)
         rows = max(int(k), 0)
         hit_ref = np.empty((self.n_q, rows), dtype=np.int32)
@@ -317,11 +344,11 @@ class BatchAligner(object):
         """Threshold search of every resident query against all resident references (ssw_engine_search_all): every hit
         (status 1 or score1 >= max(min_score, 1)).  Returns (row_off[n_q + 1] int64, hit_ref int32, hits RESULT_DTYPE,
         cigar_pool uint32) in CSR form: row q is [row_off[q], row_off[q + 1]), in ascending reference index.  More hits
-        than max_hits raise RuntimeError."""
+        than max_hits raise RuntimeError.  mat=None with query profiles resident."""
         f = self.lib.ssw_engine_search_all
         f.argtypes = [ct.c_void_p, ct.POINTER(BatchParams), ct.c_int32, ct.c_int64, ct.POINTER(ct.c_void_p)]
         f.restype = ct.c_int
-        mat, matp = _i8(mat)
+        mat, matp = _mat(mat)
         P = BatchParams(matp, n, gap_open, gap_extend, flag, filters, filterd, mask_len, score_size)
         handle = ct.c_void_p()
         rv = f(self.h, ct.byref(P), int(min_score), int(max_hits), ct.byref(handle))

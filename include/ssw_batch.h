@@ -28,7 +28,7 @@ typedef struct ssw_engine ssw_engine;
 /* Scoring and reporting parameters shared by all pairs of a batch; same meaning
  * as the arguments of ssw_init / ssw_align (ssw.h:86, :126-134). */
 typedef struct {
-	const int8_t* mat;      /* n*n scores, row = reference code, column = query code */
+	const int8_t* mat;      /* n*n scores, row = reference code, column = query code; NULL with query profiles resident */
 	int32_t n;              /* alphabet size (codes are 0..n-1), n <= 64 */
 	uint8_t gap_open;       /* weight_gapO */
 	uint8_t gap_extend;     /* weight_gapE */
@@ -87,6 +87,22 @@ int ssw_engine_set_sequences_packed(ssw_engine* e,
                                     int32_t n_queries, const int8_t* queries, const int64_t* query_off,
                                     int32_t n_refs, const uint8_t* refs_packed, const int64_t* ref_off,
                                     int32_t bits, int32_t n);
+
+/*
+ * The same with every query given as a position-specific scoring matrix (PSSM, a query profile) instead of codes: row i of
+ * query q holds the scores of query position i against the n reference letters, at pssm[(query_off[q] + i) * n + letter].
+ *   query_off   n_queries + 1 offsets in ROWS; 1 <= n <= 64; references are codes 0 .. n-1 as for ssw_engine_set_sequences
+ *   meaning     the record of query q against reference r is what the reference returns for ssw_init(read = {0, 1, .., L-1},
+ *               readLen = L, mat = M, N = max(L, n), score_size) + ssw_align(r, ...) with M[c * N + i] = P[i][c] (c < n, i < L)
+ *               and 0 elsewhere: every lookup mat[ref][read[i]] becomes P[i][ref], and the byte bias max(0, -min P) -- with it
+ *               the byte-overflow limit 255 - bias -- belongs to each query
+ *   calls       while profiles are resident, ssw_engine_align / _search / _search_all take params->mat == NULL and
+ *               params->n == n (anything else returns -1); ssw_engine_mark_mismatch returns -1 (no query letters to compare)
+ * Replaces any previously resident set; any set_sequences call after it makes query codes resident again.
+ */
+int ssw_engine_set_sequences_pssm(ssw_engine* e,
+                                  int32_t n_queries, const int8_t* pssm, const int64_t* query_off, int32_t n,
+                                  int32_t n_refs, const int8_t* refs, const int64_t* ref_off);
 
 /*
  * Align pairs of resident sequences.
