@@ -189,6 +189,7 @@ struct ssw_engine {
 	 * codes are resident).  Per query: the byte bias max(0, -min P) and the largest score, as ssw_init derives them from a matrix. */
 	int pssm_n = 0;
 	std::vector<int32_t> q_bias, q_max;
+	bool self = false;               /* ssw_engine_set_sequences_self: the queries and the references are one set (ssw_engine_search_self) */
 
 	/* scratch */
 	SswDevBuf d_items, d_bests, d_alns, d_res, d_colmax, d_tb, d_bnd, d_park, d_emul, d_grid, d_out, d_sync;
@@ -485,6 +486,7 @@ static int set_sequences_impl(ssw_engine* e,
 	if (check_offsets("reference", n_refs, ref_off, (int64_t)1 << 46, SSW_MAX_REF_LEN)) return -1;
 	SSW_CUDA_OK(cudaSetDevice(e->device));
 	e->n_q = n_queries; e->n_r = n_refs;
+	e->self = false;
 	e->from_text = false;
 	e->cached_ref_len = -1;
 	e->grid_arm_ok = true;
@@ -536,6 +538,17 @@ extern "C" int ssw_engine_set_sequences_pssm(ssw_engine* e,
 	catch (...) { return -1; }
 }
 
+extern "C" int ssw_engine_set_sequences_self(ssw_engine* e, int32_t n, const int8_t* seqs, const int64_t* off)
+{
+	try {
+		const int rc = set_sequences_impl(e, n, seqs, off, n, seqs, off);
+		if (rc == 0) e->self = true;
+		return rc;
+	}
+	catch (const std::exception& ex) { fprintf(stderr, "[libssw-b200] ssw_engine_set_sequences_self: %s\n", ex.what()); return -1; }
+	catch (...) { return -1; }
+}
+
 /* One query against one reference, as ssw_align sees it.  The reference's consumers loop over many reads against one large
  * reference (main.c:462-532, ssw_cpp.cpp:336); when the bytes at `ref` are the ones already resident (same length, same 64-bit
  * content hash) only the query is uploaded -- no host copy, no re-padding, no H2D of the reference. */
@@ -555,6 +568,7 @@ extern "C" int ssw_engine_set_pair(ssw_engine* e, const int8_t* read, int32_t re
 		SSW_CUDA_OK(cudaSetDevice(e->device));
 		e->n_q = 1;
 		e->pssm_n = 0;
+		e->self = false;
 		e->q_off.assign(2, 0); e->q_off[1] = readLen;
 		e->h_q.assign(read, read + readLen);
 		if (e->d_q.ensure(e->h_q.size() + 16)) return -1;
@@ -577,6 +591,7 @@ static int set_sequences_packed_impl(ssw_engine* e, int32_t n_queries, const int
 	e->cached_ref_len = -1;
 	e->grid_arm_ok = true;
 	e->pssm_n = 0;
+	e->self = false;
 	const int64_t qb = n_queries ? query_off[n_queries] : 0, rb = n_refs ? ref_off[n_refs] : 0;
 	e->n_q = n_queries; e->n_r = n_refs;
 	if (n_queries) e->q_off.assign(query_off, query_off + n_queries + 1); else e->q_off.assign(1, 0);
@@ -644,6 +659,7 @@ static int set_sequences_text_impl(ssw_engine* e,
 	e->cached_ref_len = -1;
 	e->grid_arm_ok = true;
 	e->pssm_n = 0;
+	e->self = false;
 	const int64_t qb = n_queries ? query_off[n_queries] : 0, rb = n_refs ? ref_off[n_refs] : 0;
 	e->n_q = n_queries * (1 + rc); e->n_r = n_refs;
 	if (n_queries) e->q_off.assign(query_off, query_off + n_queries + 1); else e->q_off.assign(1, 0);
@@ -1558,6 +1574,11 @@ struct GridSearch {
 	std::vector<ssw_batch_result> hits;     /* n_q * k */
 	std::vector<std::vector<SearchHit>> rows;   /* k == 0: n_q rows of grid hits in ascending reference index (the caller's) */
 	std::vector<uint8_t> q_on, r_on;        /* n_q, n_r: the grid path computed the pairs (q, r) with q_on[q] && r_on[r] */
+	/* self-search (k == 0, one set resident as queries and references): rank[i] is sequence i's place in canonical order; only
+	 * queries ranked in [rank_lo, rank_hi) are on the grid, and each only against the references ranked after it -- the pairs
+	 * (q, r) with q_on[q] && r_on[r] && rank[r] > rank[q] */
+	const int32_t* rank = nullptr;
+	int32_t rank_lo = 0, rank_hi = 0;
 };
 
 /* Returns 1 when the grid path handled the batch (results filled -- or, with `gs`, the hit table; `redo` lists pairs to re-do
@@ -1580,6 +1601,20 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 	std::vector<int32_t> rsel;
 	for (int r = 0; r < n_r_all; ++r) if (e->r_len[r] <= e->opt.grid_max_ref) rsel.push_back(r);
 	const int n_r = (int)rsel.size();
+	/* Self-search: the references in canonical order instead (a tile is then a range of ranks), and after[q] the first device
+	 * number ranked after sequence q -- the references q needs are [after[q], n_r).  The host sorts each row by index at the end. */
+	const bool self = gs && gs->rank;
+	std::vector<int32_t> after;
+	if (self) {
+		std::sort(rsel.begin(), rsel.end(), [&](int32_t x, int32_t y) { return gs->rank[x] < gs->rank[y]; });
+		std::vector<int32_t> canon((size_t)n_q);
+		for (int q = 0; q < n_q; ++q) canon[gs->rank[q]] = q;
+		after.assign((size_t)n_q, 0);
+		for (int t = 0, d = 0; t < n_q; ++t) {
+			if (d < n_r && rsel[d] == canon[t]) ++d;
+			after[canon[t]] = d;
+		}
+	}
 	/* The queries of the grid keep their index (the tables hold all of them; the others are in no query pair). */
 	std::vector<SswGridQ> qt((size_t)n_q);
 	std::vector<int> q_inst((size_t)n_q, -1);
@@ -1590,16 +1625,21 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 		qt[q].mask_len = P.mask_len < 0 ? len / 2 : P.mask_len;
 		qt[q].limit = S.limit_of(q, word);
 		if (len < 1) continue;
+		if (self && (gs->rank[q] < gs->rank_lo || gs->rank[q] >= gs->rank_hi)) continue;
 		if (S.has_byte && S.has_word && (int64_t)len * std::max(S.max_of(q), 0) >= 2 * (int64_t)S.limit_byte_of(q)) continue;   /* word-first prediction: general path */
 		q_inst[q] = pick_inst(qt[q].lp, e->opt.force_inst);
 		if (q_inst[q] >= 0) order.push_back(q);
 	}
 	const int n_qe = (int)order.size();
 	if (!gs && (n_r != n_r_all || n_qe != n_q)) return 0;
-	if (n_qe == 0 || (int64_t)n_qe * n_r < std::max(e->opt.grid_min_pairs, 1)) return 0;
+	int64_t grid_pairs = (int64_t)n_qe * n_r;
+	if (self) { grid_pairs = 0; for (int32_t q : order) grid_pairs += n_r - after[q]; }
+	if (n_qe == 0 || grid_pairs < std::max(e->opt.grid_min_pairs, 1)) return 0;
 	Trace tr;
+	/* self-search: query pairs of consecutive queries in canonical order within an instance, half a the earlier one */
 	std::sort(order.begin(), order.end(), [&](int32_t x, int32_t y) {
 		if (q_inst[x] != q_inst[y]) return q_inst[x] < q_inst[y];
+		if (self) return gs->rank[x] < gs->rank[y];
 		if (qt[x].lp != qt[y].lp) return qt[x].lp < qt[y].lp;
 		return x < y;
 	});
@@ -1614,7 +1654,9 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 	const bool all = gs && gs->k == 0;
 	const size_t n_slots = all ? 2 * (size_t)(n_q / 2 + 1) : 0;
 	const size_t o_scnt = o_list + (4 * (size_t)redo_cap + 255) / 256 * 256, o_soff = o_scnt + (4 * n_slots + 255) / 256 * 256;
-	if (e->d_grid.ensure(all ? o_soff + 8 * (n_slots + 1) : o_list + 4 * (size_t)redo_cap)) return -1;
+	/* self-search: behind them, the launch group's query-pair table */
+	const size_t o_sq = (o_soff + 8 * (n_slots + 1) + 255) / 256 * 256;
+	if (e->d_grid.ensure(self ? o_sq + sizeof(SswGridSelfQp) * (size_t)(n_q / 2 + 2) : all ? o_soff + 8 * (n_slots + 1) : o_list + 4 * (size_t)redo_cap)) return -1;
 	uint8_t* gb = e->d_grid.as<uint8_t>();
 	SSW_CUDA_OK(cudaMemcpyAsync(gb + o_qt, qt.data(), sizeof(SswGridQ) * n_q, cudaMemcpyHostToDevice, e->stream));
 	SSW_CUDA_OK(cudaMemsetAsync(gb + o_cnt, 0, 256, e->stream));
@@ -1720,7 +1762,7 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 		/* The order in which a query pair's items sweep the references: longest first.  The groups of a warp run until the longest
 		 * of their items is done, so neighbours of equal length waste no steps, and the longest items of a launch start first.
 		 * Stable: references of equal length keep their order (a database of one length is launched exactly as without it). */
-		if (e->opt.grid_order) std::stable_sort(perm.begin(), perm.end(), [&](int32_t x, int32_t y) { return g_len[x] > g_len[y]; });
+		if (e->opt.grid_order && !self) std::stable_sort(perm.begin(), perm.end(), [&](int32_t x, int32_t y) { return g_len[x] > g_len[y]; });
 		/* planned sweep of one query pair: group-columns of the warps (groups per warp x the warp's longest item) by groups per warp */
 		int64_t cols_useful = 0, cols_planned[3] = {0, 0, 0};                 /* 1, 2, 4 groups per warp */
 		for (int r = 0; r < n_rt; ++r) cols_useful += g_len[r];
@@ -1730,6 +1772,18 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 				for (int r = r0; r < std::min(n_rt, r0 + (1 << s)); ++r) longest = std::max(longest, g_len[perm[r]]);
 				cols_planned[s] += (int64_t)longest << s;
 			}
+		/* Self-search: slot rr sweeps reference n_rt - 1 - rr, so a query pair's live slots are a prefix [0, m) and, the lengths
+		 * not increasing along the slots, a warp's longest item is its first.  Per prefix length m: useful columns
+		 * slot_cols[m] and planned group-columns planned_pre[s][ceil(m / 2^s)] << s. */
+		std::vector<int64_t> slot_cols, planned_pre[3];
+		if (self) {
+			slot_cols.assign((size_t)n_rt + 1, 0);
+			for (int rr = 0; rr < n_rt; ++rr) slot_cols[rr + 1] = slot_cols[rr] + g_len[n_rt - 1 - rr];
+			for (int s = 0; s < 3; ++s) {
+				planned_pre[s].assign(1, 0);
+				for (int rr = 0; rr < n_rt; rr += 1 << s) planned_pre[s].push_back(planned_pre[s].back() + g_len[n_rt - 1 - rr]);
+			}
+		}
 		SSW_CUDA_OK(cudaMemcpyAsync(gb + o_roff, g_off.data(), 8 * (size_t)n_rt, cudaMemcpyHostToDevice, e->stream));
 		SSW_CUDA_OK(cudaMemcpyAsync(gb + o_rlen, g_len.data(), 4 * (size_t)n_rt, cudaMemcpyHostToDevice, e->stream));
 		SSW_CUDA_OK(cudaMemcpyAsync(gb + o_cmp, cm_prefix.data(), 8 * (size_t)n_rt, cudaMemcpyHostToDevice, e->stream));
@@ -1741,19 +1795,42 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 			const int n_r_pad = (n_rt + per_cta - 1) / per_cta * per_cta;
 			/* query pairs of this launch: same instance, bounded by memory */
 			const size_t per_qp = (size_t)cm_per_qp * 4 + (size_t)n_r_pad * (sizeof(SswItem) + sizeof(SswItemBest)) + (size_t)n_rt * 2 * (sizeof(SswAlnDesc) + sizeof(SswFillResult));
-			size_t max_qp = std::max<size_t>(1, budget / per_qp);
+			/* self-search: bounded by the query pairs' live scratch below instead */
+			size_t max_qp = self ? SIZE_MAX : std::max<size_t>(1, budget / per_qp);
 			/* large grids: several launch groups even when memory would allow one, so that the records of a finished group are
 			 * copied to the host while the next group computes (115 MB of records per million pairs) */
 			if ((int64_t)n_qe * n_r >= e->opt.grid_split_pairs)
 				max_qp = std::min<size_t>(max_qp, std::max<size_t>((size_t)std::max(e->opt.grid_group_qp, 1), ((size_t)n_qe / 2 + 7) / 8));
 			if (pilot_pending && (size_t)n_qe / 2 >= 16) max_qp = std::min<size_t>(max_qp, std::max<size_t>(2, (size_t)n_qe / 64));   /* the pilot: 1/32 of the queries */
 			std::vector<int2> qps;
+			std::vector<SswGridSelfQp> sq;              /* self-search: the launch's query-pair table, n_qp + 1 entries */
+			int64_t self_items = 0, self_cm = 0, self_live = 0, self_pairs = 0, self_useful = 0, self_planned = 0;
+			size_t self_bytes = 0;
+			const int spw = kInst[inst].G == 32 ? 0 : kInst[inst].G == 16 ? 1 : 2;   /* log2 of the groups per warp */
 			const size_t k_first = k;
 			while (k < order.size() && q_inst[order[k]] == inst && qps.size() < max_qp) {
 				int2 pr = make_int2(order[k], -1);
+				const size_t k_pr = k;
 				++k;
 				if (k < order.size() && q_inst[order[k]] == inst) { pr.y = order[k]; ++k; }
+				if (self) {
+					/* the tile's references ranked after each half, in tile numbers; a query pair with none is not launched */
+					const int32_t lo_a = std::min(std::max(after[pr.x] - r_lo, 0), n_rt);
+					const int32_t lo_b = pr.y < 0 ? n_rt : std::min(std::max(after[pr.y] - r_lo, 0), n_rt);
+					const int64_t m = n_rt - lo_a, m_pad = (m + per_cta - 1) / per_cta * per_cta, cm = cm_per_qp - (lo_a < n_rt ? cm_prefix[lo_a] : cm_per_qp);
+					if (m == 0) continue;
+					const size_t b = (size_t)cm * 4 + (size_t)m_pad * (sizeof(SswItem) + sizeof(SswItemBest)) + (size_t)m * 2 * (sizeof(SswAlnDesc) + sizeof(SswFillResult));
+					if (!qps.empty() && self_bytes + b > budget) { k = k_pr; break; }
+					self_bytes += b;
+					sq.push_back(SswGridSelfQp{self_items, self_live, self_cm, lo_a, lo_b});
+					self_items += m_pad; self_cm += cm; self_live += m; self_pairs += m + (n_rt - lo_b);
+					self_useful += slot_cols[m]; self_planned += planned_pre[spw][(m + (1 << spw) - 1) >> spw] << spw;
+				}
 				qps.push_back(pr);
+			}
+			if (self) {
+				if (qps.empty()) continue;
+				sq.push_back(SswGridSelfQp{self_items, self_live, self_cm, n_rt, n_rt});
 			}
 			SswGridArgs A;
 			A.n_qp = (int32_t)qps.size(); A.n_r = n_rt; A.n_r_pad = n_r_pad; A.word = word; A.cm_words_per_qp = cm_per_qp;
@@ -1763,20 +1840,29 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 				for (const int2& pr : qps) { lp_max = std::max(lp_max, qt[pr.x].lp); if (pr.y >= 0) lp_max = std::max(lp_max, qt[pr.y].lp); }
 				A.arm_tail = e->opt.grid_arm > 0 ? e->opt.grid_arm : lp_max / 4 + 64;
 			}
-			const int64_t n_items = (int64_t)A.n_qp * n_r_pad, n_desc = (int64_t)A.n_qp * n_rt * 2;
+			const int64_t n_items = self ? self_items : (int64_t)A.n_qp * n_r_pad, n_desc = self ? 2 * self_live : (int64_t)A.n_qp * n_rt * 2;
+			const int64_t cm_words = self ? self_cm : (int64_t)A.n_qp * cm_per_qp;
 			if (n_items > 0x7fffffff || n_desc > 0x7fffffff) return 0;
 			if (e->d_items.ensure(sizeof(SswItem) * (size_t)n_items)) return -1;
 			if (e->d_bests.ensure(sizeof(SswItemBest) * (size_t)n_items)) return -1;
 			if (e->d_alns.ensure(sizeof(SswAlnDesc) * (size_t)n_desc)) return -1;
 			if (e->d_res.ensure(sizeof(SswFillResult) * (size_t)n_desc)) return -1;
-			if (e->d_colmax.ensure((size_t)A.n_qp * (size_t)cm_per_qp * 4 + 64)) return -1;
+			if (e->d_colmax.ensure((size_t)cm_words * 4 + 64)) return -1;
 			SSW_CUDA_OK(cudaMemcpyAsync(gb + o_qp, qps.data(), sizeof(int2) * qps.size(), cudaMemcpyHostToDevice, e->stream));
+			const SswGridSelfQp* d_sq = reinterpret_cast<const SswGridSelfQp*>(gb + o_sq);
+			if (self) SSW_CUDA_OK(cudaMemcpyAsync(gb + o_sq, sq.data(), sizeof(SswGridSelfQp) * sq.size(), cudaMemcpyHostToDevice, e->stream));
 			e->laps.start(e->stream);
-			ssw_launch(ssw_grid_plan_kernel, dim3((unsigned)((n_items + 255) / 256)), dim3(256), 0, e->stream, A,
-			           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
-			           (const int64_t*)reinterpret_cast<int64_t*>(gb + o_roff), (const int32_t*)reinterpret_cast<int32_t*>(gb + o_rlen),
-			           (const int64_t*)reinterpret_cast<int64_t*>(gb + o_cmp), (const int32_t*)reinterpret_cast<int32_t*>(gb + o_perm),
-			           e->d_items.as<SswItem>(), e->d_alns.as<SswAlnDesc>());
+			if (self)
+				ssw_launch(ssw_grid_self_plan_kernel, dim3((unsigned)((n_items + 255) / 256)), dim3(256), 0, e->stream, A,
+				           (const int2*)reinterpret_cast<int2*>(gb + o_qp), d_sq, (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
+				           (const int64_t*)reinterpret_cast<int64_t*>(gb + o_roff), (const int32_t*)reinterpret_cast<int32_t*>(gb + o_rlen),
+				           (const int64_t*)reinterpret_cast<int64_t*>(gb + o_cmp), e->d_items.as<SswItem>(), e->d_alns.as<SswAlnDesc>());
+			else
+				ssw_launch(ssw_grid_plan_kernel, dim3((unsigned)((n_items + 255) / 256)), dim3(256), 0, e->stream, A,
+				           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
+				           (const int64_t*)reinterpret_cast<int64_t*>(gb + o_roff), (const int32_t*)reinterpret_cast<int32_t*>(gb + o_rlen),
+				           (const int64_t*)reinterpret_cast<int64_t*>(gb + o_cmp), (const int32_t*)reinterpret_cast<int32_t*>(gb + o_perm),
+				           e->d_items.as<SswItem>(), e->d_alns.as<SswAlnDesc>());
 			SSW_CUDA_OK(cudaGetLastError());
 			e->laps.stop(e->stream, &e->timing.resolve_ms);
 			e->timing.other_launches += 1;
@@ -1789,9 +1875,9 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 				if (rc) return rc < 0 ? rc : -1;
 				e->laps.stop(e->stream, &e->timing.fill_forward_ms);
 				e->timing.fill_forward_launches += 1;
-				e->timing.cells_forward += (int64_t)A.n_qp * (cm_per_qp) * inst_rows(inst) * 2;
-				e->timing.grid_cols_useful += (int64_t)A.n_qp * cols_useful;
-				e->timing.grid_cols_planned += (int64_t)A.n_qp * cols_planned[kInst[inst].G == 32 ? 0 : kInst[inst].G == 16 ? 1 : 2];
+				e->timing.cells_forward += cm_words * inst_rows(inst) * 2;
+				e->timing.grid_cols_useful += self ? self_useful : (int64_t)A.n_qp * cols_useful;
+				e->timing.grid_cols_planned += self ? self_planned : (int64_t)A.n_qp * cols_planned[spw];
 			}
 			e->laps.start(e->stream);
 			{
@@ -1803,6 +1889,11 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 					ssw_launch(ssw_grid_emit_kernel, dim3((unsigned)((n_desc + 255) / 256)), dim3(256), 0, e->stream, A,
 					           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
 					           (const SswFillResult*)e->d_res.as<SswFillResult>(), e->d_out.as<ssw_batch_result>(),
+					           reinterpret_cast<int32_t*>(gb + o_list), reinterpret_cast<int32_t*>(gb + o_cnt), redo_cap);
+				else if (self)
+					ssw_launch(ssw_grid_self_count_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream, A,
+					           (const int2*)reinterpret_cast<int2*>(gb + o_qp), d_sq, (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
+					           (const SswFillResult*)e->d_res.as<SswFillResult>(), gs->min_score, reinterpret_cast<int32_t*>(gb + o_scnt),
 					           reinterpret_cast<int32_t*>(gb + o_list), reinterpret_cast<int32_t*>(gb + o_cnt), redo_cap);
 				else if (all)
 					ssw_launch(ssw_grid_count_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream, A,
@@ -1844,7 +1935,7 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 				int32_t n_now = 0;
 				SSW_CUDA_OK(cudaMemcpyAsync(&n_now, gb + o_cnt, 4, cudaMemcpyDeviceToHost, e->stream));
 				SSW_CUDA_OK(cudaStreamSynchronize(e->stream));
-				pilot_pairs = (int64_t)A.n_qp * 2 * n_rt;
+				pilot_pairs = self ? self_pairs : (int64_t)A.n_qp * 2 * n_rt;
 				if ((int64_t)n_now * 500 > pilot_pairs) {    /* a re-done pair costs ~400x what arming saves per pair */
 					/* arming does not pay for these sequences: forget the pilot (its re-do list too) and run its queries again,
 					 * armed from column 0, as the first regular group -- 1/32 of the grid is computed twice, nothing goes through
@@ -1876,10 +1967,16 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 					uint8_t* hb = e->d_hits.as<uint8_t>();
 					SSW_CUDA_OK(cudaMemcpyAsync(gb + o_soff, hg.off.data(), 8 * hg.off.size(), cudaMemcpyHostToDevice, e->stream));
 					e->laps.start(e->stream);
-					ssw_launch(ssw_grid_compact_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream, A,
-					           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
-					           (const SswFillResult*)e->d_res.as<SswFillResult>(), gs->min_score, (const int64_t*)reinterpret_cast<int64_t*>(gb + o_soff),
-					           reinterpret_cast<int32_t*>(hb + o_ref), reinterpret_cast<ssw_batch_result*>(hb));
+					if (self)
+						ssw_launch(ssw_grid_self_compact_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream, A,
+						           (const int2*)reinterpret_cast<int2*>(gb + o_qp), d_sq, (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
+						           (const SswFillResult*)e->d_res.as<SswFillResult>(), gs->min_score, (const int64_t*)reinterpret_cast<int64_t*>(gb + o_soff),
+						           reinterpret_cast<int32_t*>(hb + o_ref), reinterpret_cast<ssw_batch_result*>(hb));
+					else
+						ssw_launch(ssw_grid_compact_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream, A,
+						           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
+						           (const SswFillResult*)e->d_res.as<SswFillResult>(), gs->min_score, (const int64_t*)reinterpret_cast<int64_t*>(gb + o_soff),
+						           reinterpret_cast<int32_t*>(hb + o_ref), reinterpret_cast<ssw_batch_result*>(hb));
 					SSW_CUDA_OK(cudaGetLastError());
 					e->laps.stop(e->stream, &e->timing.resolve_ms);
 					e->timing.other_launches += 1;
@@ -1901,6 +1998,8 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 	for (const GridGroup& gg : groups) if (!gg.contiguous) all_contiguous = false;
 	if (all) {
 		if (flush_hits()) return -1;                 /* the last group's hits */
+		if (self)                                    /* rows came in canonical order */
+			for (std::vector<SearchHit>& v : gs->rows) std::sort(v.begin(), v.end(), [](const SearchHit& a, const SearchHit& b) { return a.r < b.r; });
 	} else if (gs) {
 		/* the hit table in one copy (rows of a rejected pilot group were overwritten by their second run) */
 		std::vector<uint8_t> h(o_nh + 4 * (size_t)n_q);
@@ -2319,6 +2418,10 @@ static int64_t cigar_words_bound(int64_t ql, int64_t rl, int gap_extend)
 
 static bool ref_before(const SearchHit& a, const SearchHit& b) { return a.r < b.r; }
 
+/* The triangle of a self-search: the pairs (canon[i], canon[j]) with lo <= i < hi and j > i, where canon lists the sequences in
+ * canonical order (length, then index, ascending) and rank is its inverse. */
+struct SelfTri { std::vector<int32_t> rank, canon; int32_t lo, hi; };
+
 /* The rows of a search over the full grid, shared by the top-k search (keep = k: a row holds its k best hits in rank order)
  * and the threshold search (keep = 0: every hit, in ascending reference index).  The grid path takes what it can; the pairs
  * it re-does and the pairs it leaves over run through the general path and are merged into their rows (disjoint sets, so a
@@ -2326,7 +2429,7 @@ static bool ref_before(const SearchHit& a, const SearchHit& b) { return a.r < b.
  * cigar_pool or, with own_pool, to a pool sized for them.  keep = 0 and more than max_hits hits: -2. */
 static int search_rows(ssw_engine* e, const ssw_batch_params& P, int32_t keep, int32_t min_score, int64_t max_hits,
                        std::vector<std::vector<SearchHit>>& best, uint32_t* cigar_pool, int64_t pool_cap, int64_t* pool_used,
-                       std::vector<uint32_t>* own_pool)
+                       std::vector<uint32_t>* own_pool, const SelfTri* tri = nullptr)
 {
 	int64_t no_pool = 0;
 	SSW_CUDA_OK(cudaSetDevice(e->device));
@@ -2345,10 +2448,15 @@ static int search_rows(ssw_engine* e, const ssw_batch_params& P, int32_t keep, i
 	auto settle = [&](int32_t q) {
 		std::vector<SearchHit>& v = best[q];
 		if (keep > 0) keep_best(v, keep);
-		else std::inplace_merge(v.begin(), std::is_sorted_until(v.begin(), v.end(), ref_before), v.end(), ref_before);
+		else {
+			const auto mid = std::is_sorted_until(v.begin(), v.end(), ref_before);
+			if (tri) std::sort(mid, v.end(), ref_before);      /* a self-search adds a row's pairs in canonical order */
+			std::inplace_merge(v.begin(), mid, v.end(), ref_before);
+		}
 	};
 	GridSearch gs;
 	gs.k = keep; gs.min_score = thr; gs.max_hits = max_hits;
+	if (tri) { gs.rank = tri->rank.data(); gs.rank_lo = tri->lo; gs.rank_hi = tri->hi; }
 	std::vector<int64_t> redo;
 	int rc = grid_scores(e, P0, S, (int64_t)n_q * n_r, nullptr, &redo, &gs);
 	if (rc < 0) return rc;
@@ -2379,19 +2487,28 @@ static int search_rows(ssw_engine* e, const ssw_batch_params& P, int32_t keep, i
 	}
 	/* The pairs the grid did not take -- a query off the grid against every reference, a query on it against the references off
 	 * it -- go through the general path in blocks of whole queries and are merged per query in the same way; the selection of
-	 * these is on the host.  Memory is bounded by a block. */
+	 * these is on the host.  Memory is bounded by a block.  A self-search takes its queries in canonical order, each against the
+	 * references ranked after it only. */
 	std::vector<int32_t> r_off_grid;
 	for (int32_t r = 0; r < n_r; ++r) if (!gs.r_on[r]) r_off_grid.push_back(r);
 	std::vector<int32_t> pq, pr;
 	std::vector<ssw_batch_result> rec;
-	for (int32_t q0 = 0; q0 < n_q;) {
+	const int32_t i_end = tri ? tri->hi : n_q;
+	auto q_at = [&](int32_t i) { return tri ? tri->canon[i] : i; };
+	for (int32_t q0 = tri ? tri->lo : 0; q0 < i_end;) {
 		int32_t q1 = q0;
 		pq.clear(); pr.clear();
-		for (; q1 < n_q; ++q1) {
-			const int64_t row = gs.q_on[q1] ? (int64_t)r_off_grid.size() : n_r;
+		for (; q1 < i_end; ++q1) {
+			const int32_t q = q_at(q1);
+			const int64_t row = gs.q_on[q] ? (int64_t)r_off_grid.size() : tri ? n_r - 1 - q1 : n_r;
 			if (q1 > q0 && (int64_t)pq.size() + row > SSW_SEARCH_BLOCK_PAIRS) break;
-			if (gs.q_on[q1]) for (int32_t r : r_off_grid) { pq.push_back(q1); pr.push_back(r); }
-			else for (int32_t r = 0; r < n_r; ++r) { pq.push_back(q1); pr.push_back(r); }
+			if (gs.q_on[q]) { for (int32_t r : r_off_grid) if (!tri || tri->rank[r] > q1) { pq.push_back(q); pr.push_back(r); } }
+			else if (tri) {
+				/* an empty sequence comes first in canonical order and is the query of all its pairs: it aligns nowhere (score 0),
+				 * so none of them is a hit, and none is computed */
+				if (e->q_off[q + 1] > e->q_off[q]) for (int32_t j = q1 + 1; j < n_r; ++j) { pq.push_back(q); pr.push_back(tri->canon[j]); }
+			}
+			else for (int32_t r = 0; r < n_r; ++r) { pq.push_back(q); pr.push_back(r); }
 		}
 		const int64_t m = (int64_t)pq.size();
 		if (m > 0) {
@@ -2404,7 +2521,7 @@ static int search_rows(ssw_engine* e, const ssw_batch_params& P, int32_t keep, i
 			e->timing.leftover_pairs += m;
 			for (int64_t i = 0; i < m; ++i) if (is_hit(rec[i], thr)) { best[pq[i]].push_back(SearchHit{pr[i], rec[i]}); ++n_kept; }
 			if (keep == 0 && n_kept > max_hits) return -2;
-			for (int32_t q = q0; q < q1; ++q) settle(q);
+			for (int32_t i = q0; i < q1; ++i) settle(q_at(i));
 		}
 		q0 = q1;
 	}
@@ -2480,6 +2597,21 @@ extern "C" int ssw_engine_search(ssw_engine* e, const ssw_batch_params* params, 
 /* threshold search over the full grid: every hit, as a CSR matrix in pair order                  */
 /* ------------------------------------------------------------------------------------------- */
 
+/* the rows of search_rows as the CSR matrix of a hit set (pool already in place); empties the rows */
+static void fill_hit_set(std::vector<std::vector<SearchHit>>& best, ssw_hit_set* s)
+{
+	s->n_rows = (int32_t)best.size();
+	s->row_off.assign(best.size() + 1, 0);
+	for (size_t q = 0; q < best.size(); ++q) s->row_off[q + 1] = s->row_off[q] + (int64_t)best[q].size();
+	const size_t n = (size_t)s->row_off.back();
+	s->hit_ref.resize(n); s->hits.resize(n);
+	size_t j = 0;
+	for (std::vector<SearchHit>& v : best) {
+		for (const SearchHit& h : v) { s->hit_ref[j] = h.r; s->hits[j] = h.rec; ++j; }
+		std::vector<SearchHit>().swap(v);
+	}
+}
+
 static int engine_search_all_impl(ssw_engine* e, const ssw_batch_params* params, int32_t min_score, int64_t max_hits, ssw_hit_set** out)
 {
 	if (!out) { fprintf(stderr, "[libssw-b200] ssw_engine_search_all: NULL output\n"); return -1; }
@@ -2495,16 +2627,7 @@ static int engine_search_all_impl(ssw_engine* e, const ssw_batch_params* params,
 	const int rc = search_rows(e, P, 0, min_score, max_hits, best, nullptr, 0, &used, &s->pool);
 	if (rc == -2) fprintf(stderr, "[libssw-b200] ssw_engine_search_all: more than max_hits = %lld hits\n", (long long)max_hits);
 	if (rc) return rc;
-	s->n_rows = e->n_q;
-	s->row_off.assign((size_t)e->n_q + 1, 0);
-	for (int32_t q = 0; q < e->n_q; ++q) s->row_off[q + 1] = s->row_off[q] + (int64_t)best[q].size();
-	const size_t n = (size_t)s->row_off.back();
-	s->hit_ref.resize(n); s->hits.resize(n);
-	size_t j = 0;
-	for (std::vector<SearchHit>& v : best) {
-		for (const SearchHit& h : v) { s->hit_ref[j] = h.r; s->hits[j] = h.rec; ++j; }
-		std::vector<SearchHit>().swap(v);
-	}
+	fill_hit_set(best, s.get());
 	*out = s.release();
 	return 0;
 }
@@ -2515,6 +2638,64 @@ extern "C" int ssw_engine_search_all(ssw_engine* e, const ssw_batch_params* para
 	try { SswBusyGuard busy(e ? e->device : 0); return engine_search_all_impl(e, params, min_score, max_hits, out); }
 	catch (const std::exception& ex) { fprintf(stderr, "[libssw-b200] ssw_engine_search_all: %s\n", ex.what()); return -1; }
 	catch (...) { return -1; }
+}
+
+/* ------------------------------------------------------------------------------------------- */
+/* self-search: every pair of one set above a threshold, each unordered pair computed once        */
+/* ------------------------------------------------------------------------------------------- */
+
+/* With a symmetric matrix and gap_open > gap_extend the score of a pair does not depend on which sequence is the query, so the
+ * pair {i, j} is computed once, as query = the earlier of the two in canonical order (length, then index, ascending).  The
+ * queries ranked in [rank_lo, rank_hi) only (the device groups' share); rows of the others stay empty. */
+int ssw_engine_search_self_ranks(ssw_engine* e, const ssw_batch_params* params, int32_t min_score, int64_t max_hits,
+                                 int32_t rank_lo, int32_t rank_hi, ssw_hit_set** out)
+{
+	if (out) *out = nullptr;
+	try {
+		SswBusyGuard busy(e ? e->device : 0);
+		if (!out) { fprintf(stderr, "[libssw-b200] ssw_engine_search_self: NULL output\n"); return -1; }
+		if (!e || !params) { fprintf(stderr, "[libssw-b200] ssw_engine_search_self: no engine or no parameters\n"); return -1; }
+		if (!e->self) { fprintf(stderr, "[libssw-b200] ssw_engine_search_self: the resident sequences were not set by ssw_engine_set_sequences_self\n"); return -1; }
+		const ssw_batch_params& P = *params;
+		if (!P.mat) { fprintf(stderr, "[libssw-b200] ssw_engine_search_self: no scoring matrix (params->mat is NULL)\n"); return -1; }
+		if (P.n < 1 || P.n > 64) { fprintf(stderr, "[libssw-b200] alphabet size %d not supported (1..64)\n", P.n); return -1; }
+		if (max_hits < 0) { fprintf(stderr, "[libssw-b200] ssw_engine_search_self: max_hits = %lld is negative\n", (long long)max_hits); return -1; }
+		if (P.gap_open <= P.gap_extend) {
+			fprintf(stderr, "[libssw-b200] ssw_engine_search_self: gap_open %d <= gap_extend %d: scores are not symmetric\n", P.gap_open, P.gap_extend);
+			return -1;
+		}
+		for (int a = 0; a < P.n; ++a)
+			for (int b = 0; b < a; ++b)
+				if (P.mat[a * P.n + b] != P.mat[b * P.n + a]) {
+					fprintf(stderr, "[libssw-b200] ssw_engine_search_self: the matrix is not symmetric (%d, %d)\n", a, b);
+					return -1;
+				}
+		const int32_t n = e->n_q;
+		SelfTri tri;
+		tri.canon.resize((size_t)n); tri.rank.resize((size_t)n);
+		for (int32_t i = 0; i < n; ++i) tri.canon[i] = i;
+		std::sort(tri.canon.begin(), tri.canon.end(), [&](int32_t x, int32_t y) { return e->r_len[x] != e->r_len[y] ? e->r_len[x] < e->r_len[y] : x < y; });
+		for (int32_t t = 0; t < n; ++t) tri.rank[tri.canon[t]] = t;
+		tri.lo = std::max(rank_lo, 0); tri.hi = std::min(rank_hi, n);
+		std::unique_ptr<ssw_hit_set> s(new ssw_hit_set());
+		std::vector<std::vector<SearchHit>> best((size_t)n);
+		if (tri.lo < tri.hi) {
+			int64_t used = 0;
+			const int rc = search_rows(e, P, 0, min_score, max_hits, best, nullptr, 0, &used, &s->pool, &tri);
+			if (rc == -2) fprintf(stderr, "[libssw-b200] ssw_engine_search_self: more than max_hits = %lld hits\n", (long long)max_hits);
+			if (rc) return rc;
+		}
+		fill_hit_set(best, s.get());
+		*out = s.release();
+		return 0;
+	}
+	catch (const std::exception& ex) { fprintf(stderr, "[libssw-b200] ssw_engine_search_self: %s\n", ex.what()); return -1; }
+	catch (...) { return -1; }
+}
+
+extern "C" int ssw_engine_search_self(ssw_engine* e, const ssw_batch_params* params, int32_t min_score, int64_t max_hits, ssw_hit_set** out)
+{
+	return ssw_engine_search_self_ranks(e, params, min_score, max_hits, 0, e ? e->n_q : 0, out);
 }
 
 extern "C" int ssw_hit_set_view(const ssw_hit_set* s, ssw_hit_view* v)

@@ -382,4 +382,118 @@ ssw_grid_compact_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGri
 	}
 }
 
+/* ---- self-search (ssw_engine_search_self): the pairs of one set above the diagonal of its canonical order -------------- */
+
+/* One query pair of a self-search launch.  The device numbers the tile's references in canonical order (length, then index,
+ * ascending) and slot rr of every query pair sweeps reference n_r - 1 - rr (longest first).  Half a needs the references
+ * [lo_a, n_r) -- those ranked after its query, the live slots [0, n_r - lo_a) -- and half b, the later query of the pair,
+ * [lo_b, n_r) with lo_b >= lo_a.  Items, descriptors (two per live slot, at desc0 + r - lo_a) and column maxima (cm0 +
+ * cm_prefix[r] - cm_prefix[lo_a]) are ragged: item0 is the launch's prefix of the live slots, each query pair's padded to
+ * whole CTAs, and entry n_qp of the table holds the launch's item count. */
+struct SswGridSelfQp { int64_t item0, desc0, cm0; int32_t lo_a, lo_b; };
+
+/* thread idx -> item (query pair found by binary search over item0, slot rr): as ssw_grid_plan_kernel over the live slots */
+__global__ void __launch_bounds__(256)
+ssw_grid_self_plan_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGridSelfQp* __restrict__ sq, const SswGridQ* __restrict__ qt,
+                          const int64_t* __restrict__ ref_off, const int32_t* __restrict__ ref_len, const int64_t* __restrict__ cm_prefix,
+                          SswItem* __restrict__ items, SswAlnDesc* __restrict__ descs)
+{
+	const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (idx >= sq[A.n_qp].item0) return;
+	int pi = 0;
+	for (int hi = A.n_qp - 1; pi < hi;) {
+		const int m = (pi + hi + 1) >> 1;
+		if (sq[m].item0 <= idx) pi = m; else hi = m - 1;
+	}
+	const SswGridSelfQp s = sq[pi];
+	const int rr = (int)(idx - s.item0);
+	const bool live = rr < A.n_r - s.lo_a;
+	const int r = A.n_r - 1 - (live ? rr : 0);
+	const int2 pr = qp[pi];
+	const SswGridQ qa = qt[pr.x];
+	SswItem it;
+	it.qa.off = qa.off; it.qa.len = qa.len; it.qa.lp = qa.lp; it.qa.rev = 0;
+	it.qb.off = 0; it.qb.len = 0; it.qb.lp = 0; it.qb.rev = 0;
+	SswGridQ qb;
+	qb.off = 0; qb.len = 0; qb.lp = 0; qb.mask_len = 0; qb.limit = 0;
+	if (pr.y >= 0) { qb = qt[pr.y]; it.qb.off = qb.off; it.qb.len = qb.len; it.qb.lp = qb.lp; }
+	it.ref_off = ref_off[r]; it.ref_len = ref_len[r];
+	it.cend = (A.arm_tail > 0 && live) ? max(0, ref_len[r] - A.arm_tail) : 0;
+	it.p0 = 0; it.p1 = live ? ref_len[r] : 0; it.warm = 0; it.term_a = -1;
+	it.cm_off = live ? s.cm0 + cm_prefix[r] - cm_prefix[s.lo_a] : SSW_CM_NONE;
+	items[idx] = it;
+	if (live) {
+		SswAlnDesc d;
+		d.first_item = (int32_t)idx; d.n_items = 1; d.half = 0; d.ref_len = it.ref_len; d.read_len = qa.len;
+		d.word = A.word; d.limit = qa.limit; d.mask_len = qa.mask_len; d.cm_off = it.cm_off; d.scan_all = 0; d.warm = 0; d.byte_pad = 0;
+		const int64_t di = (s.desc0 + r - s.lo_a) * 2;
+		descs[di] = d;
+		d.half = 1; d.read_len = qb.len; d.mask_len = qb.mask_len; d.limit = qb.limit;
+		if (pr.y < 0 || r < s.lo_b) d.n_items = 0;                     /* no second query, or not ranked after it: skipped */
+		descs[di + 1] = d;
+	}
+}
+
+/* ssw_grid_count_kernel over the references of the slot's half only: [lo_a, n_r) or [lo_b, n_r) */
+__global__ void __launch_bounds__(SSW_SELECT_THREADS)
+ssw_grid_self_count_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGridSelfQp* __restrict__ sq, const SswGridQ* __restrict__ qt,
+                           const SswFillResult* __restrict__ res, int32_t min_score, int32_t* __restrict__ slot_n,
+                           int32_t* __restrict__ redo_list, int32_t* __restrict__ redo_count, int32_t redo_cap)
+{
+	__shared__ int32_t s_n;
+	const int h = (int)(blockIdx.x & 1), pi = (int)(blockIdx.x >> 1);
+	const int2 pr = qp[pi];
+	const int q = h ? pr.y : pr.x;
+	const int tid = threadIdx.x;
+	if (q < 0) {
+		if (tid == 0) slot_n[blockIdx.x] = 0;
+		return;
+	}
+	const SswGridSelfQp s = sq[pi];
+	const int mask_len = qt[q].mask_len;
+	const int n_r = A.n_r;
+	const int64_t d0 = s.desc0 - s.lo_a, p0 = (int64_t)q * n_r;          /* result of reference r: res[2 * (d0 + r) + h] */
+	if (tid == 0) s_n = 0;
+	__syncthreads();
+	int c = 0;
+	for (int r = (h ? s.lo_b : s.lo_a) + tid; r < n_r; r += SSW_SELECT_THREADS) {
+		ssw_batch_result o;
+		if (ssw_grid_record<true>(res[2 * (d0 + r) + h], mask_len, p0 + r, o, redo_list, redo_count, redo_cap) && o.score1 >= min_score) ++c;
+	}
+	if (c) atomicAdd(&s_n, c);
+	__syncthreads();
+	if (tid == 0) slot_n[blockIdx.x] = s_n;
+}
+
+/* ssw_grid_compact_kernel over the same references */
+__global__ void __launch_bounds__(SSW_SELECT_THREADS)
+ssw_grid_self_compact_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGridSelfQp* __restrict__ sq, const SswGridQ* __restrict__ qt,
+                             const SswFillResult* __restrict__ res, int32_t min_score, const int64_t* __restrict__ slot_off,
+                             int32_t* __restrict__ hit_ref, ssw_batch_result* __restrict__ hits)
+{
+	__shared__ int32_t s_warp[2][SSW_SELECT_THREADS / 32];
+	const int h = (int)(blockIdx.x & 1), pi = (int)(blockIdx.x >> 1);
+	const int2 pr = qp[pi];
+	const int q = h ? pr.y : pr.x;
+	if (q < 0) return;
+	const SswGridSelfQp s = sq[pi];
+	const int mask_len = qt[q].mask_len;
+	const int n_r = A.n_r, tid = threadIdx.x;
+	const int64_t d0 = s.desc0 - s.lo_a, p0 = (int64_t)q * n_r;
+	const int64_t base = slot_off[blockIdx.x], cnt = slot_off[blockIdx.x + 1] - base;
+	int64_t done = 0;
+	for (int r0 = h ? s.lo_b : s.lo_a, it = 0; r0 < n_r && done < cnt; r0 += SSW_SELECT_THREADS, ++it) {
+		const int r = r0 + tid;
+		ssw_batch_result o;
+		const bool hit = r < n_r && ssw_grid_record<false>(res[2 * (d0 + r) + h], mask_len, p0 + r, o, nullptr, nullptr, 0) && o.score1 >= min_score;
+		int n = 0;
+		const int at = ssw_block_prefix(hit, s_warp[it & 1], &n);
+		if (hit) {
+			hits[base + done + at] = o;
+			hit_ref[base + done + at] = r;
+		}
+		done += n;
+	}
+}
+
 #endif /* SSW_GRID_CUH */

@@ -486,6 +486,94 @@ extern "C" int ssw_group_search_all(ssw_group* g, const ssw_batch_params* params
 	catch (...) { return -1; }
 }
 
+extern "C" int ssw_group_search_self(ssw_group* g, const ssw_batch_params* params, int32_t n, const int8_t* seqs, const int64_t* off,
+                                     int32_t min_score, int64_t max_hits, ssw_hit_set** out)
+{
+	if (!out) { fprintf(stderr, "[libssw-b200] ssw_group_search_self: NULL output\n"); return -1; }
+	*out = nullptr;
+	if (!g || g->eng.empty() || !params) { fprintf(stderr, "[libssw-b200] ssw_group_search_self: NULL argument\n"); return -1; }
+	if (n < 0 || (n > 0 && (!seqs || !off))) { fprintf(stderr, "[libssw-b200] ssw_group_search_self: no sequences\n"); return -1; }
+	struct Part {
+		ssw_hit_set* set = nullptr;
+		int rc = 0;
+		Part() = default;
+		Part(const Part&) = delete;
+		Part& operator=(const Part&) = delete;
+		~Part() { ssw_hit_set_destroy(set); }
+	};
+	try {
+		for (int32_t i = 0; i < n; ++i) if (off[i + 1] < off[i]) { fprintf(stderr, "[libssw-b200] offsets are not non-decreasing at %d\n", i); return -1; }
+		/* canonical order (length, then index) and the triangle cells of each rank: its length times the letters ranked after it */
+		std::vector<int32_t> canon((size_t)n), rank((size_t)n);
+		for (int32_t i = 0; i < n; ++i) canon[i] = i;
+		auto len = [&](int32_t i) { return off[i + 1] - off[i]; };
+		std::sort(canon.begin(), canon.end(), [&](int32_t x, int32_t y) { return len(x) != len(y) ? len(x) < len(y) : x < y; });
+		for (int32_t t = 0; t < n; ++t) rank[canon[t]] = t;
+		std::vector<long double> cells((size_t)n);
+		long double later = 0;
+		for (int32_t t = n - 1; t >= 0; --t) { cells[t] = (long double)len(canon[t]) * later; later += len(canon[t]); }
+		const int world = (int)g->eng.size();
+		const std::vector<int64_t> b = balanced_bounds(n, world, [&](int64_t t) { return cells[t]; });
+		std::vector<Part> parts((size_t)world);
+		auto work = [&](int d) {
+			Part& S = parts[d];
+			try {
+				ssw_engine* e = g->eng[d];
+				S.rc = ssw_engine_set_sequences_self(e, n, seqs, off);
+				if (S.rc) return;
+				S.rc = ssw_engine_search_self_ranks(e, params, min_score, max_hits, (int32_t)b[d], (int32_t)b[d + 1], &S.set);
+			}
+			catch (const std::exception& ex) { fprintf(stderr, "[libssw-b200] device group: %s\n", ex.what()); S.rc = -1; }
+			catch (...) { S.rc = -1; }
+		};
+#ifdef SSW_CPU_EMU
+		for (int d = 0; d < world; ++d) work(d);        /* the emulator's fibers are not thread-safe */
+#else
+		{
+			std::vector<std::thread> th;
+			th.reserve((size_t)world);
+			for (int d = 1; d < world; ++d) {
+				try { th.emplace_back(work, d); }
+				catch (...) { work(d); }
+			}
+			work(0);
+			for (std::thread& t : th) t.join();
+		}
+#endif
+		for (const Part& S : parts) if (S.rc) return S.rc;
+		int64_t n_hits = 0, n_words = 0;
+		for (const Part& S : parts) { n_hits += (int64_t)S.set->hits.size(); n_words += (int64_t)S.set->pool.size(); }
+		if (n_hits > max_hits) { fprintf(stderr, "[libssw-b200] ssw_group_search_self: more than max_hits = %lld hits\n", (long long)max_hits); return -2; }
+		if (n_words > 0x7fffffff) { fprintf(stderr, "[libssw-b200] more than 2^31 CIGAR words in one batch: split the batch\n"); return -1; }
+		/* row i comes from the device whose rank range holds rank[i] */
+		std::unique_ptr<ssw_hit_set> s(new ssw_hit_set());
+		s->n_rows = n;
+		s->row_off.reserve((size_t)n + 1);
+		s->row_off.push_back(0);
+		s->hit_ref.reserve((size_t)n_hits); s->hits.reserve((size_t)n_hits); s->pool.reserve((size_t)n_words);
+		std::vector<int64_t> base((size_t)world, 0);
+		for (int d = 0; d < world; ++d) {
+			base[d] = (int64_t)s->pool.size();
+			s->pool.insert(s->pool.end(), parts[d].set->pool.begin(), parts[d].set->pool.end());
+		}
+		for (int32_t i = 0; i < n; ++i) {
+			const int d = (int)(std::upper_bound(b.begin(), b.end(), (int64_t)rank[i]) - b.begin()) - 1;
+			const ssw_hit_set& S = *parts[d].set;
+			for (int64_t j = S.row_off[i]; j < S.row_off[i + 1]; ++j) {
+				ssw_batch_result o = S.hits[j];
+				if (o.cigar_off >= 0) o.cigar_off += (int32_t)base[d];
+				s->hits.push_back(o);
+				s->hit_ref.push_back(S.hit_ref[j]);
+			}
+			s->row_off.push_back((int64_t)s->hits.size());
+		}
+		*out = s.release();
+		return 0;
+	}
+	catch (const std::exception& ex) { fprintf(stderr, "[libssw-b200] ssw_group_search_self: %s\n", ex.what()); return -1; }
+	catch (...) { return -1; }
+}
+
 extern "C" int ssw_group_align_batch(ssw_group* g, const ssw_batch_params* params, const int8_t* table, int32_t add_reverse_complement,
                                      int32_t n_queries, const void* queries, const int64_t* query_off,
                                      int32_t n_refs, const void* refs, const int64_t* ref_off,

@@ -15,4 +15,9 @@ struct ssw_hit_set {
 	std::vector<uint32_t> pool;               /* CIGAR words of the hits (flag & 7) */
 };
 
+/* ssw_engine_search_self for the queries of canonical ranks [rank_lo, rank_hi) only (ssw_group_search_self: one range per
+ * device); the set still has a row for every resident sequence, those of the other queries empty. */
+int ssw_engine_search_self_ranks(ssw_engine* e, const ssw_batch_params* params, int32_t min_score, int64_t max_hits,
+                                 int32_t rank_lo, int32_t rank_hi, ssw_hit_set** out);
+
 #endif

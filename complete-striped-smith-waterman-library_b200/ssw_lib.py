@@ -206,6 +206,19 @@ class BatchAligner(object):
         self.n_q, self.n_r = len(queries), len(refs)
         self._lens = (np.diff(qo), np.diff(ro))
 
+    def set_sequences_self(self, seqs):
+        """One set (list of int8 code arrays) resident as both the queries and the references (ssw_engine_set_sequences_self):
+        align / search / search_all then give what they give after set_sequences(seqs, seqs), and search_self runs."""
+        c, o = concat(seqs)
+        f = self.lib.ssw_engine_set_sequences_self
+        f.argtypes = [ct.c_void_p, ct.c_int32, ct.POINTER(ct.c_int8), ct.POINTER(ct.c_int64)]
+        f.restype = ct.c_int
+        rv = f(self.h, len(seqs), c.ctypes.data_as(ct.POINTER(ct.c_int8)), o.ctypes.data_as(ct.POINTER(ct.c_int64)))
+        if rv:
+            raise RuntimeError("ssw_engine_set_sequences_self failed (%d)" % rv)
+        self.n_q = self.n_r = len(seqs)
+        self._lens = (np.diff(o), np.diff(o))
+
     def set_profiles(self, profiles, refs, n):
         """Host -> device copy of query profiles (PSSMs) and references (ssw_engine_set_sequences_pssm): `profiles` is a list of
         (L_q, n) int8 arrays, row i = the scores of query position i against the n reference letters; `refs` int8 code arrays.
@@ -353,6 +366,21 @@ class BatchAligner(object):
         handle = ct.c_void_p()
         rv = f(self.h, ct.byref(P), int(min_score), int(max_hits), ct.byref(handle))
         return _take_hit_set(self.lib, rv, handle, "ssw_engine_search_all", max_hits)
+
+    def search_self(self, mat, n, min_score, max_hits=SEARCH_ALL_MAX_HITS, gap_open=3, gap_extend=1, flag=0, filters=0, filterd=0,
+                    mask_len=-1, score_size=2):
+        """Self-search of the set made resident by set_sequences_self (ssw_engine_search_self): every unordered pair {i, j},
+        i != j, once, as the record of query = the earlier in canonical order (length, then index) against the other, kept by
+        the rule of search_all.  Returns (row_off[n + 1], hit_ref, hits, cigar_pool) as search_all: row i holds the hits in
+        which i is the query, in ascending partner index.  Needs a symmetric matrix and gap_open > gap_extend."""
+        f = self.lib.ssw_engine_search_self
+        f.argtypes = [ct.c_void_p, ct.POINTER(BatchParams), ct.c_int32, ct.c_int64, ct.POINTER(ct.c_void_p)]
+        f.restype = ct.c_int
+        mat, matp = _mat(mat)
+        P = BatchParams(matp, n, gap_open, gap_extend, flag, filters, filterd, mask_len, score_size)
+        handle = ct.c_void_p()
+        rv = f(self.h, ct.byref(P), int(min_score), int(max_hits), ct.byref(handle))
+        return _take_hit_set(self.lib, rv, handle, "ssw_engine_search_self", max_hits)
 
     def mark_mismatch(self, res, pool, pair_query=None, pair_ref=None):
         """mark_mismatch (ssw.c:1019-1074) for every CIGAR of a batch, on the device (ssw_engine_mark_mismatch): `res` / `pool`
@@ -581,3 +609,19 @@ class GroupAligner(object):
                qo.ctypes.data_as(ct.POINTER(ct.c_int64)), len(refs), rc.ctypes.data_as(ct.c_void_p), ro.ctypes.data_as(ct.POINTER(ct.c_int64)),
                int(min_score), int(max_hits), ct.byref(handle))
         return _take_hit_set(self.lib, rv, handle, "ssw_group_search_all", max_hits)
+
+    def search_self(self, seqs, mat, n, min_score, max_hits=SEARCH_ALL_MAX_HITS, gap_open=3, gap_extend=1, flag=0, filters=0,
+                    filterd=0, mask_len=-1, score_size=2):
+        """BatchAligner.search_self over the devices of the group (ssw_group_search_self): every device holds the whole set
+        (list of int8 code arrays) and takes a range of canonical ranks as queries.  Returns (row_off, hit_ref, hits, cigar_pool)."""
+        f = self.lib.ssw_group_search_self
+        f.argtypes = [ct.c_void_p, ct.POINTER(BatchParams), ct.c_int32, ct.POINTER(ct.c_int8), ct.POINTER(ct.c_int64),
+                      ct.c_int32, ct.c_int64, ct.POINTER(ct.c_void_p)]
+        f.restype = ct.c_int
+        mat, matp = _mat(mat)
+        P = BatchParams(matp, n, gap_open, gap_extend, flag, filters, filterd, mask_len, score_size)
+        c, o = concat(seqs)
+        handle = ct.c_void_p()
+        rv = f(self.h, ct.byref(P), len(seqs), c.ctypes.data_as(ct.POINTER(ct.c_int8)), o.ctypes.data_as(ct.POINTER(ct.c_int64)),
+               int(min_score), int(max_hits), ct.byref(handle))
+        return _take_hit_set(self.lib, rv, handle, "ssw_group_search_self", max_hits)

@@ -181,6 +181,28 @@ int ssw_hit_set_view(const ssw_hit_set* s, ssw_hit_view* v);
 void ssw_hit_set_destroy(ssw_hit_set* s);
 
 /*
+ * Self-search: every pair of ONE set that scores at or above a threshold, each unordered pair computed once.
+ *   set_sequences_self  makes seqs (n sequences, offsets off[n + 1]) resident as both the queries and the references;
+ *              afterwards ssw_engine_align / _search / _search_all give exactly what they give after
+ *              ssw_engine_set_sequences(seqs, seqs).  Any other ssw_engine_set_sequences* call ends self mode.
+ *   order      canonical order: by (length, index), ascending
+ *   pairs      each unordered pair {i, j}, i != j, at most once, as the record of query = the earlier of the two in canonical
+ *              order (the shorter; on equal lengths the smaller index) against reference = the other -- field for field what
+ *              ssw_engine_align returns for that oriented pair with the same params.  Self-pairs are not reported.
+ *   hit        as ssw_engine_search_all: status 1, or score1 >= max(min_score, 1)
+ *   output     an ssw_hit_set with n rows: row i holds the hits in which i is the query, in ascending partner index.
+ *              max_hits, the -2 return and the flag pass (begins and CIGARs for the hits only, into the set's pool) are
+ *              those of ssw_engine_search_all.
+ *   refused    (-1, *out NULL) gap_open <= gap_extend, a matrix that is not symmetric on codes < n, mat == NULL, or a resident
+ *              set that did not come from ssw_engine_set_sequences_self (profiles included).  With a symmetric matrix and
+ *              gap_open > gap_extend a pair scores the same in both orientations, so the hits and their mirrors are exactly
+ *              ssw_engine_search_all on (seqs, seqs) with the diagonal removed, at about half the work.
+ * On the device path each query pair sweeps only the references ranked after its queries (DESIGN.md section 4.4f).
+ */
+int ssw_engine_set_sequences_self(ssw_engine* e, int32_t n, const int8_t* seqs, const int64_t* off);
+int ssw_engine_search_self(ssw_engine* e, const ssw_batch_params* params, int32_t min_score, int64_t max_hits, ssw_hit_set** out);
+
+/*
  * mark_mismatch (ssw.h:157-164; ssw.c:1019-1074) for the CIGARs of a whole batch, on the device: for every record of
  * `results` that carries a CIGAR (words at cigar_pool[cigar_off ...]) the M runs are split into '=' and 'X' runs, soft
  * clips are added for the unaligned ends of the read, and nm[p] (may be NULL) receives the number of mismatching +
@@ -276,6 +298,12 @@ int ssw_group_search_all(ssw_group* g, const ssw_batch_params* params, const int
                          int32_t n_queries, const void* queries, const int64_t* query_off,
                          int32_t n_refs, const void* refs, const int64_t* ref_off,
                          int32_t min_score, int64_t max_hits, ssw_hit_set** out);
+
+/* ssw_engine_search_self over the devices of the group: every device holds the whole set and takes a contiguous range of
+ * canonical ranks as queries, cut so that the devices have nearly equal triangle cells; rows of the n sequences are
+ * concatenated and the CIGAR pools re-based.  max_hits bounds the total.  Results do not depend on the number of devices. */
+int ssw_group_search_self(ssw_group* g, const ssw_batch_params* params, int32_t n, const int8_t* seqs, const int64_t* off,
+                          int32_t min_score, int64_t max_hits, ssw_hit_set** out);
 
 /* The same with heap s_align records (ssw_align_batch / _text / _marked over a group); release with align_destroy. */
 int ssw_group_align_batch(ssw_group* g, const ssw_batch_params* params, const int8_t* table, int32_t add_reverse_complement,
