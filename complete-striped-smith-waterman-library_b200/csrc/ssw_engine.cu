@@ -1601,19 +1601,20 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 	std::vector<int32_t> rsel;
 	for (int r = 0; r < n_r_all; ++r) if (e->r_len[r] <= e->opt.grid_max_ref) rsel.push_back(r);
 	const int n_r = (int)rsel.size();
-	/* Self-search: the references in canonical order instead (a tile is then a range of ranks), and after[q] the first device
-	 * number ranked after sequence q -- the references q needs are [after[q], n_r).  The host sorts each row by index at the end. */
+	/* after[q]: the first device number query q is paired with -- the references q needs are [after[q], n_r) -- and after[n_q]
+	 * that of a missing second query.  Self-search: the references in canonical order instead (a tile is then a range of ranks),
+	 * and after[q] the first device number ranked after sequence q.  The host sorts each row by index at the end. */
 	const bool self = gs && gs->rank;
-	std::vector<int32_t> after;
+	std::vector<int32_t> after((size_t)n_q + 1, 0);
 	if (self) {
 		std::sort(rsel.begin(), rsel.end(), [&](int32_t x, int32_t y) { return gs->rank[x] < gs->rank[y]; });
 		std::vector<int32_t> canon((size_t)n_q);
 		for (int q = 0; q < n_q; ++q) canon[gs->rank[q]] = q;
-		after.assign((size_t)n_q, 0);
 		for (int t = 0, d = 0; t < n_q; ++t) {
 			if (d < n_r && rsel[d] == canon[t]) ++d;
 			after[canon[t]] = d;
 		}
+		after[n_q] = n_r;
 	}
 	/* The queries of the grid keep their index (the tables hold all of them; the others are in no query pair). */
 	std::vector<SswGridQ> qt((size_t)n_q);
@@ -1632,8 +1633,8 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 	}
 	const int n_qe = (int)order.size();
 	if (!gs && (n_r != n_r_all || n_qe != n_q)) return 0;
-	int64_t grid_pairs = (int64_t)n_qe * n_r;
-	if (self) { grid_pairs = 0; for (int32_t q : order) grid_pairs += n_r - after[q]; }
+	int64_t grid_pairs = 0;
+	for (int32_t q : order) grid_pairs += n_r - after[q];
 	if (n_qe == 0 || grid_pairs < std::max(e->opt.grid_min_pairs, 1)) return 0;
 	Trace tr;
 	/* self-search: query pairs of consecutive queries in canonical order within an instance, half a the earlier one */
@@ -1648,15 +1649,13 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 	const size_t o_qt = 0, o_roff = o_qt + (sizeof(SswGridQ) * n_q + 255) / 256 * 256, o_rlen = o_roff + (8 * (size_t)n_r + 255) / 256 * 256;
 	const size_t o_cmp = o_rlen + (4 * (size_t)n_r + 255) / 256 * 256, o_perm = o_cmp + (8 * (size_t)n_r + 255) / 256 * 256;
 	const size_t o_qp = o_perm + (4 * (size_t)n_r + 255) / 256 * 256;
-	const size_t o_cnt = o_qp + (8 * (size_t)(n_q / 2 + 1) + 255) / 256 * 256, o_list = o_cnt + 256;
+	const size_t o_cnt = o_qp + (sizeof(SswGridQp) * (size_t)(n_q / 2 + 2) + 255) / 256 * 256, o_list = o_cnt + 256;
 	const int32_t redo_cap = (int32_t)std::min<int64_t>((int64_t)n_qe * n_r, 1 << 22);
 	/* threshold search: behind the redo list, the hit counts of a launch group's query slots and their exclusive prefix */
 	const bool all = gs && gs->k == 0;
 	const size_t n_slots = all ? 2 * (size_t)(n_q / 2 + 1) : 0;
 	const size_t o_scnt = o_list + (4 * (size_t)redo_cap + 255) / 256 * 256, o_soff = o_scnt + (4 * n_slots + 255) / 256 * 256;
-	/* self-search: behind them, the launch group's query-pair table */
-	const size_t o_sq = (o_soff + 8 * (n_slots + 1) + 255) / 256 * 256;
-	if (e->d_grid.ensure(self ? o_sq + sizeof(SswGridSelfQp) * (size_t)(n_q / 2 + 2) : all ? o_soff + 8 * (n_slots + 1) : o_list + 4 * (size_t)redo_cap)) return -1;
+	if (e->d_grid.ensure(all ? o_soff + 8 * (n_slots + 1) : o_list + 4 * (size_t)redo_cap)) return -1;
 	uint8_t* gb = e->d_grid.as<uint8_t>();
 	SSW_CUDA_OK(cudaMemcpyAsync(gb + o_qt, qt.data(), sizeof(SswGridQ) * n_q, cudaMemcpyHostToDevice, e->stream));
 	SSW_CUDA_OK(cudaMemsetAsync(gb + o_cnt, 0, 256, e->stream));
@@ -1749,39 +1748,35 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 	bool arm_on = e->opt.grid_arm > 0 || (e->opt.grid_arm < 0 && P.n > 8 && e->grid_arm_ok);
 	bool pilot_pending = arm_on && e->opt.grid_arm < 0;
 	int64_t pilot_pairs = 0;
+	/* The order in which a query pair's slots sweep a tile's references: ascending slot_key, stable.  Longest first: the groups
+	 * of a warp run until the longest of their items is done, so neighbours of equal length waste no steps, and the longest
+	 * items of a launch start first; references of equal length keep their order (a database of one length is launched exactly
+	 * as without it).  Self-search: the canonical order reversed, so that the references a query pair needs, those ranked after
+	 * its queries, are a prefix of its slots. */
+	std::vector<int64_t> slot_key((size_t)n_r, 0);
+	for (int r = 0; r < n_r; ++r) slot_key[r] = self ? -r : e->opt.grid_order ? -(int64_t)e->r_len[rsel[r]] : 0;
 	for (size_t t = 0; t < n_tiles; ++t) {
 		const int32_t r_lo = tile_lo[t], n_rt = tile_lo[t + 1] - r_lo;
-		/* the tile's reference tables: its references numbered 0 .. n_rt - 1 */
-		std::vector<int64_t> cm_prefix((size_t)n_rt), g_off((size_t)n_rt);
+		/* the tile's reference tables: its references numbered 0 .. n_rt - 1 (cm_prefix[n_rt]: the column-maximum words of all) */
+		std::vector<int64_t> cm_prefix((size_t)n_rt + 1, 0), g_off((size_t)n_rt);
 		std::vector<int32_t> g_len((size_t)n_rt), perm((size_t)n_rt);
-		int64_t cm_per_qp = 0;
 		for (int r = 0; r < n_rt; ++r) {
 			g_off[r] = e->r_off[rsel[r_lo + r]]; g_len[r] = e->r_len[rsel[r_lo + r]]; perm[r] = r;
-			cm_prefix[r] = cm_per_qp; cm_per_qp += ((int64_t)g_len[r] + 3) / 4 * 4;
+			cm_prefix[r + 1] = cm_prefix[r] + ((int64_t)g_len[r] + 3) / 4 * 4;
 		}
-		/* The order in which a query pair's items sweep the references: longest first.  The groups of a warp run until the longest
-		 * of their items is done, so neighbours of equal length waste no steps, and the longest items of a launch start first.
-		 * Stable: references of equal length keep their order (a database of one length is launched exactly as without it). */
-		if (e->opt.grid_order && !self) std::stable_sort(perm.begin(), perm.end(), [&](int32_t x, int32_t y) { return g_len[x] > g_len[y]; });
-		/* planned sweep of one query pair: group-columns of the warps (groups per warp x the warp's longest item) by groups per warp */
-		int64_t cols_useful = 0, cols_planned[3] = {0, 0, 0};                 /* 1, 2, 4 groups per warp */
-		for (int r = 0; r < n_rt; ++r) cols_useful += g_len[r];
-		for (int s = 0; s < 3; ++s)
-			for (int r0 = 0; r0 < n_rt; r0 += 1 << s) {
-				int32_t longest = 0;
-				for (int r = r0; r < std::min(n_rt, r0 + (1 << s)); ++r) longest = std::max(longest, g_len[perm[r]]);
-				cols_planned[s] += (int64_t)longest << s;
-			}
-		/* Self-search: slot rr sweeps reference n_rt - 1 - rr, so a query pair's live slots are a prefix [0, m) and, the lengths
-		 * not increasing along the slots, a warp's longest item is its first.  Per prefix length m: useful columns
-		 * slot_cols[m] and planned group-columns planned_pre[s][ceil(m / 2^s)] << s. */
-		std::vector<int64_t> slot_cols, planned_pre[3];
-		if (self) {
-			slot_cols.assign((size_t)n_rt + 1, 0);
-			for (int rr = 0; rr < n_rt; ++rr) slot_cols[rr + 1] = slot_cols[rr] + g_len[n_rt - 1 - rr];
-			for (int s = 0; s < 3; ++s) {
-				planned_pre[s].assign(1, 0);
-				for (int rr = 0; rr < n_rt; rr += 1 << s) planned_pre[s].push_back(planned_pre[s].back() + g_len[n_rt - 1 - rr]);
+		std::stable_sort(perm.begin(), perm.end(), [&](int32_t x, int32_t y) { return slot_key[r_lo + x] < slot_key[r_lo + y]; });
+		/* The planned sweep of a query pair whose live slots are the first m: useful columns useful_pre[m], and group-columns of
+		 * the warps (groups per warp x the warp's longest item) planned_pre[s][m] with 2^s groups per warp (1, 2, 4). */
+		std::vector<int64_t> useful_pre((size_t)n_rt + 1, 0), planned_pre[3];
+		for (int rr = 0; rr < n_rt; ++rr) useful_pre[rr + 1] = useful_pre[rr] + g_len[perm[rr]];
+		for (int s = 0; s < 3; ++s) {
+			planned_pre[s].assign((size_t)n_rt + 1, 0);
+			int64_t warps = 0;                       /* the warps that are complete in the first rr slots */
+			int32_t longest = 0;                     /* the longest slot of the warp that is not */
+			for (int rr = 0; rr < n_rt; ++rr) {
+				longest = std::max(longest, g_len[perm[rr]]);
+				planned_pre[s][rr + 1] = (warps + longest) << s;
+				if (((rr + 1) & ((1 << s) - 1)) == 0) { warps += longest; longest = 0; }
 			}
 		}
 		SSW_CUDA_OK(cudaMemcpyAsync(gb + o_roff, g_off.data(), 8 * (size_t)n_rt, cudaMemcpyHostToDevice, e->stream));
@@ -1792,77 +1787,61 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 		while (k < order.size()) {
 			const int inst = q_inst[order[k]];
 			const int per_cta = fill_items_per_cta(inst, P.n);
-			const int n_r_pad = (n_rt + per_cta - 1) / per_cta * per_cta;
-			/* query pairs of this launch: same instance, bounded by memory */
-			const size_t per_qp = (size_t)cm_per_qp * 4 + (size_t)n_r_pad * (sizeof(SswItem) + sizeof(SswItemBest)) + (size_t)n_rt * 2 * (sizeof(SswAlnDesc) + sizeof(SswFillResult));
-			/* self-search: bounded by the query pairs' live scratch below instead */
-			size_t max_qp = self ? SIZE_MAX : std::max<size_t>(1, budget / per_qp);
+			/* query pairs of this launch: same instance, bounded by memory (their live scratch, below) */
+			size_t max_qp = SIZE_MAX;
 			/* large grids: several launch groups even when memory would allow one, so that the records of a finished group are
 			 * copied to the host while the next group computes (115 MB of records per million pairs) */
 			if ((int64_t)n_qe * n_r >= e->opt.grid_split_pairs)
 				max_qp = std::min<size_t>(max_qp, std::max<size_t>((size_t)std::max(e->opt.grid_group_qp, 1), ((size_t)n_qe / 2 + 7) / 8));
 			if (pilot_pending && (size_t)n_qe / 2 >= 16) max_qp = std::min<size_t>(max_qp, std::max<size_t>(2, (size_t)n_qe / 64));   /* the pilot: 1/32 of the queries */
-			std::vector<int2> qps;
-			std::vector<SswGridSelfQp> sq;              /* self-search: the launch's query-pair table, n_qp + 1 entries */
-			int64_t self_items = 0, self_cm = 0, self_live = 0, self_pairs = 0, self_useful = 0, self_planned = 0;
-			size_t self_bytes = 0;
+			std::vector<SswGridQp> qps;                 /* the launch's query-pair table; n_qp + 1 entries once complete */
+			int64_t n_items = 0, n_live = 0, cm_words = 0, pairs = 0, cols_useful = 0, cols_planned = 0;
+			size_t bytes = 0;
 			const int spw = kInst[inst].G == 32 ? 0 : kInst[inst].G == 16 ? 1 : 2;   /* log2 of the groups per warp */
 			const size_t k_first = k;
 			while (k < order.size() && q_inst[order[k]] == inst && qps.size() < max_qp) {
-				int2 pr = make_int2(order[k], -1);
+				SswGridQp s;
 				const size_t k_pr = k;
-				++k;
-				if (k < order.size() && q_inst[order[k]] == inst) { pr.y = order[k]; ++k; }
-				if (self) {
-					/* the tile's references ranked after each half, in tile numbers; a query pair with none is not launched */
-					const int32_t lo_a = std::min(std::max(after[pr.x] - r_lo, 0), n_rt);
-					const int32_t lo_b = pr.y < 0 ? n_rt : std::min(std::max(after[pr.y] - r_lo, 0), n_rt);
-					const int64_t m = n_rt - lo_a, m_pad = (m + per_cta - 1) / per_cta * per_cta, cm = cm_per_qp - (lo_a < n_rt ? cm_prefix[lo_a] : cm_per_qp);
-					if (m == 0) continue;
-					const size_t b = (size_t)cm * 4 + (size_t)m_pad * (sizeof(SswItem) + sizeof(SswItemBest)) + (size_t)m * 2 * (sizeof(SswAlnDesc) + sizeof(SswFillResult));
-					if (!qps.empty() && self_bytes + b > budget) { k = k_pr; break; }
-					self_bytes += b;
-					sq.push_back(SswGridSelfQp{self_items, self_live, self_cm, lo_a, lo_b});
-					self_items += m_pad; self_cm += cm; self_live += m; self_pairs += m + (n_rt - lo_b);
-					self_useful += slot_cols[m]; self_planned += planned_pre[spw][(m + (1 << spw) - 1) >> spw] << spw;
-				}
-				qps.push_back(pr);
+				s.qa = order[k++]; s.qb = -1;
+				if (k < order.size() && q_inst[order[k]] == inst) s.qb = order[k++];
+				/* the tile's references each half needs, in tile numbers; a query pair with none is not launched */
+				s.lo_a = std::min(std::max(after[s.qa] - r_lo, 0), n_rt);
+				s.lo_b = std::min(std::max(after[s.qb < 0 ? n_q : s.qb] - r_lo, 0), n_rt);
+				const int64_t m = n_rt - s.lo_a, m_pad = (m + per_cta - 1) / per_cta * per_cta, cm = cm_prefix[n_rt] - cm_prefix[s.lo_a];
+				if (m == 0) continue;
+				const size_t b = (size_t)cm * 4 + (size_t)m_pad * (sizeof(SswItem) + sizeof(SswItemBest)) + (size_t)m * 2 * (sizeof(SswAlnDesc) + sizeof(SswFillResult));
+				if (!qps.empty() && bytes + b > budget) { k = k_pr; break; }
+				bytes += b;
+				s.item0 = n_items; s.desc0 = n_live; s.cm0 = cm_words;
+				qps.push_back(s);
+				n_items += m_pad; n_live += m; cm_words += cm; pairs += m + (n_rt - s.lo_b);
+				cols_useful += useful_pre[m]; cols_planned += planned_pre[spw][m];
 			}
-			if (self) {
-				if (qps.empty()) continue;
-				sq.push_back(SswGridSelfQp{self_items, self_live, self_cm, n_rt, n_rt});
-			}
+			if (qps.empty()) continue;
 			SswGridArgs A;
-			A.n_qp = (int32_t)qps.size(); A.n_r = n_rt; A.n_r_pad = n_r_pad; A.word = word; A.cm_words_per_qp = cm_per_qp;
+			A.n_qp = (int32_t)qps.size(); A.n_r = n_rt; A.word = word;
 			A.arm_tail = 0;
 			if (arm_on) {
 				int lp_max = 0;
-				for (const int2& pr : qps) { lp_max = std::max(lp_max, qt[pr.x].lp); if (pr.y >= 0) lp_max = std::max(lp_max, qt[pr.y].lp); }
+				for (const SswGridQp& s : qps) { lp_max = std::max(lp_max, qt[s.qa].lp); if (s.qb >= 0) lp_max = std::max(lp_max, qt[s.qb].lp); }
 				A.arm_tail = e->opt.grid_arm > 0 ? e->opt.grid_arm : lp_max / 4 + 64;
 			}
-			const int64_t n_items = self ? self_items : (int64_t)A.n_qp * n_r_pad, n_desc = self ? 2 * self_live : (int64_t)A.n_qp * n_rt * 2;
-			const int64_t cm_words = self ? self_cm : (int64_t)A.n_qp * cm_per_qp;
+			qps.push_back(SswGridQp{-1, -1, n_rt, n_rt, n_items, n_live, cm_words});
+			const int64_t n_desc = 2 * n_live;
 			if (n_items > 0x7fffffff || n_desc > 0x7fffffff) return 0;
 			if (e->d_items.ensure(sizeof(SswItem) * (size_t)n_items)) return -1;
 			if (e->d_bests.ensure(sizeof(SswItemBest) * (size_t)n_items)) return -1;
 			if (e->d_alns.ensure(sizeof(SswAlnDesc) * (size_t)n_desc)) return -1;
 			if (e->d_res.ensure(sizeof(SswFillResult) * (size_t)n_desc)) return -1;
 			if (e->d_colmax.ensure((size_t)cm_words * 4 + 64)) return -1;
-			SSW_CUDA_OK(cudaMemcpyAsync(gb + o_qp, qps.data(), sizeof(int2) * qps.size(), cudaMemcpyHostToDevice, e->stream));
-			const SswGridSelfQp* d_sq = reinterpret_cast<const SswGridSelfQp*>(gb + o_sq);
-			if (self) SSW_CUDA_OK(cudaMemcpyAsync(gb + o_sq, sq.data(), sizeof(SswGridSelfQp) * sq.size(), cudaMemcpyHostToDevice, e->stream));
+			SSW_CUDA_OK(cudaMemcpyAsync(gb + o_qp, qps.data(), sizeof(SswGridQp) * qps.size(), cudaMemcpyHostToDevice, e->stream));
+			const SswGridQp* d_qp = reinterpret_cast<const SswGridQp*>(gb + o_qp);
 			e->laps.start(e->stream);
-			if (self)
-				ssw_launch(ssw_grid_self_plan_kernel, dim3((unsigned)((n_items + 255) / 256)), dim3(256), 0, e->stream, A,
-				           (const int2*)reinterpret_cast<int2*>(gb + o_qp), d_sq, (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
-				           (const int64_t*)reinterpret_cast<int64_t*>(gb + o_roff), (const int32_t*)reinterpret_cast<int32_t*>(gb + o_rlen),
-				           (const int64_t*)reinterpret_cast<int64_t*>(gb + o_cmp), e->d_items.as<SswItem>(), e->d_alns.as<SswAlnDesc>());
-			else
-				ssw_launch(ssw_grid_plan_kernel, dim3((unsigned)((n_items + 255) / 256)), dim3(256), 0, e->stream, A,
-				           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
-				           (const int64_t*)reinterpret_cast<int64_t*>(gb + o_roff), (const int32_t*)reinterpret_cast<int32_t*>(gb + o_rlen),
-				           (const int64_t*)reinterpret_cast<int64_t*>(gb + o_cmp), (const int32_t*)reinterpret_cast<int32_t*>(gb + o_perm),
-				           e->d_items.as<SswItem>(), e->d_alns.as<SswAlnDesc>());
+			ssw_launch(ssw_grid_plan_kernel, dim3((unsigned)((n_items + 255) / 256)), dim3(256), 0, e->stream, A,
+			           d_qp, (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
+			           (const int64_t*)reinterpret_cast<int64_t*>(gb + o_roff), (const int32_t*)reinterpret_cast<int32_t*>(gb + o_rlen),
+			           (const int64_t*)reinterpret_cast<int64_t*>(gb + o_cmp), (const int32_t*)reinterpret_cast<int32_t*>(gb + o_perm),
+			           e->d_items.as<SswItem>(), e->d_alns.as<SswAlnDesc>());
 			SSW_CUDA_OK(cudaGetLastError());
 			e->laps.stop(e->stream, &e->timing.resolve_ms);
 			e->timing.other_launches += 1;
@@ -1876,8 +1855,8 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 				e->laps.stop(e->stream, &e->timing.fill_forward_ms);
 				e->timing.fill_forward_launches += 1;
 				e->timing.cells_forward += cm_words * inst_rows(inst) * 2;
-				e->timing.grid_cols_useful += self ? self_useful : (int64_t)A.n_qp * cols_useful;
-				e->timing.grid_cols_planned += self ? self_planned : (int64_t)A.n_qp * cols_planned[spw];
+				e->timing.grid_cols_useful += cols_useful;
+				e->timing.grid_cols_planned += cols_planned;
 			}
 			e->laps.start(e->stream);
 			{
@@ -1887,30 +1866,25 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 				           (const uint32_t*)e->d_colmax.as<uint32_t>(), e->d_res.as<SswFillResult>());
 				if (!gs)
 					ssw_launch(ssw_grid_emit_kernel, dim3((unsigned)((n_desc + 255) / 256)), dim3(256), 0, e->stream, A,
-					           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
+					           d_qp, (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
 					           (const SswFillResult*)e->d_res.as<SswFillResult>(), e->d_out.as<ssw_batch_result>(),
-					           reinterpret_cast<int32_t*>(gb + o_list), reinterpret_cast<int32_t*>(gb + o_cnt), redo_cap);
-				else if (self)
-					ssw_launch(ssw_grid_self_count_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream, A,
-					           (const int2*)reinterpret_cast<int2*>(gb + o_qp), d_sq, (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
-					           (const SswFillResult*)e->d_res.as<SswFillResult>(), gs->min_score, reinterpret_cast<int32_t*>(gb + o_scnt),
 					           reinterpret_cast<int32_t*>(gb + o_list), reinterpret_cast<int32_t*>(gb + o_cnt), redo_cap);
 				else if (all)
 					ssw_launch(ssw_grid_count_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream, A,
-					           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
+					           d_qp, (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
 					           (const SswFillResult*)e->d_res.as<SswFillResult>(), gs->min_score, reinterpret_cast<int32_t*>(gb + o_scnt),
 					           reinterpret_cast<int32_t*>(gb + o_list), reinterpret_cast<int32_t*>(gb + o_cnt), redo_cap);
 				else {
 					/* the first tile selects into the running table; a later tile into the tile table, merged into the running one */
 					uint8_t* hb = e->d_hits.as<uint8_t>(), *tb = hb + (t ? o_tile : 0);
 					ssw_launch(ssw_grid_select_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream, A,
-					           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
+					           d_qp, (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
 					           (const SswFillResult*)e->d_res.as<SswFillResult>(), gs->k, gs->min_score,
 					           reinterpret_cast<int32_t*>(tb + o_href), reinterpret_cast<ssw_batch_result*>(tb), reinterpret_cast<int32_t*>(tb + o_nh),
 					           reinterpret_cast<int32_t*>(gb + o_list), reinterpret_cast<int32_t*>(gb + o_cnt), redo_cap);
 					if (t) {
 						ssw_launch(ssw_grid_merge_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream,
-						           (const int2*)reinterpret_cast<int2*>(gb + o_qp), gs->k, r_lo,
+						           d_qp, gs->k, r_lo,
 						           reinterpret_cast<int32_t*>(hb + o_href), reinterpret_cast<ssw_batch_result*>(hb), reinterpret_cast<int32_t*>(hb + o_nh),
 						           (const int32_t*)reinterpret_cast<int32_t*>(tb + o_href), (const ssw_batch_result*)reinterpret_cast<ssw_batch_result*>(tb),
 						           (const int32_t*)reinterpret_cast<int32_t*>(tb + o_nh));
@@ -1935,7 +1909,7 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 				int32_t n_now = 0;
 				SSW_CUDA_OK(cudaMemcpyAsync(&n_now, gb + o_cnt, 4, cudaMemcpyDeviceToHost, e->stream));
 				SSW_CUDA_OK(cudaStreamSynchronize(e->stream));
-				pilot_pairs = self ? self_pairs : (int64_t)A.n_qp * 2 * n_rt;
+				pilot_pairs = pairs;
 				if ((int64_t)n_now * 500 > pilot_pairs) {    /* a re-done pair costs ~400x what arming saves per pair */
 					/* arming does not pay for these sequences: forget the pilot (its re-do list too) and run its queries again,
 					 * armed from column 0, as the first regular group -- 1/32 of the grid is computed twice, nothing goes through
@@ -1957,7 +1931,7 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 				SSW_CUDA_OK(cudaMemcpyAsync(sn.data(), gb + o_scnt, 4 * sn.size(), cudaMemcpyDeviceToHost, e->stream));
 				SSW_CUDA_OK(cudaStreamSynchronize(e->stream));
 				hg.off.assign(sn.size() + 1, 0); hg.q.resize(sn.size()); hg.r_lo = r_lo;
-				for (size_t s = 0; s < sn.size(); ++s) { hg.q[s] = s & 1 ? qps[s / 2].y : qps[s / 2].x; hg.off[s + 1] = hg.off[s] + sn[s]; }
+				for (size_t s = 0; s < sn.size(); ++s) { hg.q[s] = s & 1 ? qps[s / 2].qb : qps[s / 2].qa; hg.off[s + 1] = hg.off[s] + sn[s]; }
 				hg.n = hg.off.back();
 				grid_hits += hg.n;
 				if (grid_hits > gs->max_hits) return -2;
@@ -1967,16 +1941,10 @@ static int grid_scores(ssw_engine* e, const ssw_batch_params& P, const Sem& S, i
 					uint8_t* hb = e->d_hits.as<uint8_t>();
 					SSW_CUDA_OK(cudaMemcpyAsync(gb + o_soff, hg.off.data(), 8 * hg.off.size(), cudaMemcpyHostToDevice, e->stream));
 					e->laps.start(e->stream);
-					if (self)
-						ssw_launch(ssw_grid_self_compact_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream, A,
-						           (const int2*)reinterpret_cast<int2*>(gb + o_qp), d_sq, (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
-						           (const SswFillResult*)e->d_res.as<SswFillResult>(), gs->min_score, (const int64_t*)reinterpret_cast<int64_t*>(gb + o_soff),
-						           reinterpret_cast<int32_t*>(hb + o_ref), reinterpret_cast<ssw_batch_result*>(hb));
-					else
-						ssw_launch(ssw_grid_compact_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream, A,
-						           (const int2*)reinterpret_cast<int2*>(gb + o_qp), (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
-						           (const SswFillResult*)e->d_res.as<SswFillResult>(), gs->min_score, (const int64_t*)reinterpret_cast<int64_t*>(gb + o_soff),
-						           reinterpret_cast<int32_t*>(hb + o_ref), reinterpret_cast<ssw_batch_result*>(hb));
+					ssw_launch(ssw_grid_compact_kernel, dim3((unsigned)(2 * A.n_qp)), dim3(SSW_SELECT_THREADS), 0, e->stream, A,
+					           d_qp, (const SswGridQ*)reinterpret_cast<SswGridQ*>(gb + o_qt),
+					           (const SswFillResult*)e->d_res.as<SswFillResult>(), gs->min_score, (const int64_t*)reinterpret_cast<int64_t*>(gb + o_soff),
+					           reinterpret_cast<int32_t*>(hb + o_ref), reinterpret_cast<ssw_batch_result*>(hb));
 					SSW_CUDA_OK(cudaGetLastError());
 					e->laps.stop(e->stream, &e->timing.resolve_ms);
 					e->timing.other_launches += 1;

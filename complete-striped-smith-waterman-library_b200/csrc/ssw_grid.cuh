@@ -10,6 +10,8 @@
  * ssw_batch_result records.  Pairs whose byte-semantics score overflowed are appended to a list and re-done by the
  * general path.  A top-k search (ssw_engine_search) replaces the emit kernel by a selection kernel that keeps only each
  * query's k best records; a threshold search (ssw_engine_search_all) by a count and a compaction kernel that keep every hit.
+ * Six kernels -- plan, emit, select, merge (top-k over grid tiles), count and compact -- read one query-pair table
+ * (SswGridQp), which describes a full grid and a self-search's triangle (ssw_engine_search_self) alike.
  */
 #ifndef SSW_GRID_CUH
 #define SSW_GRID_CUH
@@ -24,47 +26,59 @@ struct SswGridQ { int32_t off, len, lp, mask_len, limit; };
 struct SswGridArgs {
 	int32_t n_qp;        /* query pairs in this launch */
 	int32_t n_r;         /* references */
-	int32_t n_r_pad;     /* references rounded up to a whole number of CTAs (dead items in between) */
 	int32_t word;
 	int32_t arm_tail;    /* > 0: best-cell rows are recorded in the last arm_tail columns of every reference only (SswItem.cend) */
-	int64_t cm_words_per_qp;
 };
 
-/* thread idx -> item (qp, slot rr): writes the fill item and, for live items, the two alignment descriptors.
- * Slot rr of a query pair sweeps reference perm[rr] (the host orders the slots by length, so that the groups of a warp, which
- * run as long as their longest item, end together); descriptors, column maxima and with them the resolve results stay at the
- * reference's own position r, so nothing after the fill knows about the order of the launch. */
+/* One query pair of a launch: queries qa and qb (-1: none) and their first references, lo_a and lo_b (lo_a <= lo_b).  Slot rr of
+ * the pair sweeps reference perm[rr]; the host orders the slots so that the references half a needs, [lo_a, n_r), are the slots
+ * [0, n_r - lo_a) -- the live slots -- and half b needs [lo_b, n_r).  A full grid has lo_a = lo_b = 0; a self-search, whose
+ * references are in canonical order and swept in reverse, the references ranked after each half's query.  The pair's items
+ * start at item0 (its live slots padded to whole CTAs), the descriptors of reference r at 2 (desc0 + r - lo_a) and its column
+ * maxima at cm0 + cm_prefix[r] - cm_prefix[lo_a].  Entry n_qp of the table holds the launch's totals in item0, desc0 and cm0. */
+struct SswGridQp { int32_t qa, qb, lo_a, lo_b; int64_t item0, desc0, cm0; };
+
+/* thread idx -> item (query pair found by binary search over item0, slot rr): writes the fill item and, for live slots, the two
+ * alignment descriptors.  Slots are ordered by length where the host can (the groups of a warp, which run as long as their
+ * longest item, then end together); descriptors, column maxima and with them the resolve results stay at the reference's own
+ * position r, so nothing after the fill knows about the order of the launch.  A dead slot repeats the last live slot's
+ * reference with no columns. */
 __global__ void __launch_bounds__(256)
-ssw_grid_plan_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGridQ* __restrict__ qt,
+ssw_grid_plan_kernel(SswGridArgs A, const SswGridQp* __restrict__ qp, const SswGridQ* __restrict__ qt,
                      const int64_t* __restrict__ ref_off, const int32_t* __restrict__ ref_len, const int64_t* __restrict__ cm_prefix,
                      const int32_t* __restrict__ perm, SswItem* __restrict__ items, SswAlnDesc* __restrict__ descs)
 {
 	const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-	if (idx >= (int64_t)A.n_qp * A.n_r_pad) return;
-	const int pi = (int)(idx / A.n_r_pad), rr = (int)(idx % A.n_r_pad);
-	const bool live = rr < A.n_r;
-	const int r = perm[live ? rr : A.n_r - 1];
-	const int2 pr = qp[pi];
-	const SswGridQ qa = qt[pr.x];
+	if (idx >= qp[A.n_qp].item0) return;
+	int pi = 0;
+	for (int hi = A.n_qp - 1; pi < hi;) {
+		const int m = (pi + hi + 1) >> 1;
+		if (qp[m].item0 <= idx) pi = m; else hi = m - 1;
+	}
+	const SswGridQp s = qp[pi];
+	const int rr = (int)(idx - s.item0), n_live = A.n_r - s.lo_a;
+	const bool live = rr < n_live;
+	const int r = perm[live ? rr : n_live - 1];
+	const SswGridQ qa = qt[s.qa];
 	SswItem it;
 	it.qa.off = qa.off; it.qa.len = qa.len; it.qa.lp = qa.lp; it.qa.rev = 0;
 	it.qb.off = 0; it.qb.len = 0; it.qb.lp = 0; it.qb.rev = 0;
 	SswGridQ qb;
 	qb.off = 0; qb.len = 0; qb.lp = 0; qb.mask_len = 0; qb.limit = 0;
-	if (pr.y >= 0) { qb = qt[pr.y]; it.qb.off = qb.off; it.qb.len = qb.len; it.qb.lp = qb.lp; }
+	if (s.qb >= 0) { qb = qt[s.qb]; it.qb.off = qb.off; it.qb.len = qb.len; it.qb.lp = qb.lp; }
 	it.ref_off = ref_off[r]; it.ref_len = ref_len[r];
 	it.cend = (A.arm_tail > 0 && live) ? max(0, ref_len[r] - A.arm_tail) : 0;
 	it.p0 = 0; it.p1 = live ? ref_len[r] : 0; it.warm = 0; it.term_a = -1;
-	it.cm_off = live ? (int64_t)pi * A.cm_words_per_qp + cm_prefix[r] : SSW_CM_NONE;
+	it.cm_off = live ? s.cm0 + cm_prefix[r] - cm_prefix[s.lo_a] : SSW_CM_NONE;
 	items[idx] = it;
 	if (live) {
 		SswAlnDesc d;
 		d.first_item = (int32_t)idx; d.n_items = 1; d.half = 0; d.ref_len = it.ref_len; d.read_len = qa.len;
 		d.word = A.word; d.limit = qa.limit; d.mask_len = qa.mask_len; d.cm_off = it.cm_off; d.scan_all = 0; d.warm = 0; d.byte_pad = 0;
-		const int64_t di = ((int64_t)pi * A.n_r + r) * 2;
+		const int64_t di = (s.desc0 + r - s.lo_a) * 2;
 		descs[di] = d;
 		d.half = 1; d.read_len = qb.len; d.mask_len = qb.mask_len; d.limit = qb.limit;
-		if (pr.y < 0) d.n_items = 0;                                   /* no second query: the resolve kernel skips it */
+		if (s.qb < 0 || r < s.lo_b) d.n_items = 0;                      /* no second query, or a reference it does not need: skipped */
 		descs[di + 1] = d;
 	}
 }
@@ -93,9 +107,10 @@ __device__ __forceinline__ bool ssw_grid_record(const SswFillResult& f, int mask
 	return true;
 }
 
-/* resolve result -> ssw_batch_result of pair (query, reference); overflowed byte results are queued for a re-run */
+/* resolve result -> ssw_batch_result of pair (query, reference); overflowed byte results are queued for a re-run.  An align's
+ * grid is full: descriptor di belongs to query pair di / (2 n_r). */
 __global__ void __launch_bounds__(256)
-ssw_grid_emit_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGridQ* __restrict__ qt,
+ssw_grid_emit_kernel(SswGridArgs A, const SswGridQp* __restrict__ qp, const SswGridQ* __restrict__ qt,
                      const SswFillResult* __restrict__ res, ssw_batch_result* __restrict__ out,
                      int32_t* __restrict__ redo_list, int32_t* __restrict__ redo_count, int32_t redo_cap)
 {
@@ -104,14 +119,31 @@ ssw_grid_emit_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGridQ*
 	const int h = (int)(di & 1);
 	const int64_t pt = di >> 1;
 	const int pi = (int)(pt / A.n_r), r = (int)(pt % A.n_r);
-	const int2 pr = qp[pi];
-	const int q = h ? pr.y : pr.x;
+	const int q = h ? qp[pi].qb : qp[pi].qa;
 	if (q < 0) return;
 	const SswFillResult f = res[di];
 	const int64_t p = (int64_t)q * A.n_r + r;
 	ssw_batch_result o;
 	ssw_grid_record<true>(f, qt[q].mask_len, p, o, redo_list, redo_count, redo_cap);
 	out[p] = o;
+}
+
+/* The query slot (pi, half) of CTA blockIdx.x in the selection, count and compaction kernels: its query q (-1: none), the
+ * query's mask_len, and the references it needs, [r0, n_r), whose resolve results are rq[2 r] and pair numbers p0 + r. */
+struct SswGridSlot { int q, mask_len, r0; const SswFillResult* rq; int64_t p0; };
+
+__device__ __forceinline__ SswGridSlot ssw_grid_slot(int n_r, const SswGridQp* __restrict__ qp, const SswGridQ* __restrict__ qt,
+                                                     const SswFillResult* __restrict__ res)
+{
+	const int h = (int)(blockIdx.x & 1);
+	const SswGridQp* s = qp + (blockIdx.x >> 1);
+	SswGridSlot o;
+	o.q = h ? s->qb : s->qa;
+	o.mask_len = o.q >= 0 ? qt[o.q].mask_len : 0;
+	o.r0 = h ? s->lo_b : s->lo_a;
+	o.rq = res + 2 * (s->desc0 - s->lo_a) + h;
+	o.p0 = (int64_t)o.q * n_r;
+	return o;
 }
 
 /* ---- top-k selection (ssw_engine_search) ------------------------------------------------------------------------------ */
@@ -152,12 +184,13 @@ __device__ __forceinline__ int ssw_hist_cut(const int32_t* hist, int want, int* 
 /* One CTA per query slot (pi, half) of a launch group: the k best hits of that query among the group's resolve results,
  * written to row q of the n_q x k hit table in rank order (score1 descending, reference ascending).  A hit is a pair whose
  * result is final on the grid (not re-done) with score1 >= min_score (>= 1).  Pairs to re-do are queued as the emit kernel
- * queues them and take no part in the selection; the host merges their records in afterwards.
+ * queues them and take no part in the selection; the host merges their records in afterwards.  A top-k search's grid is full
+ * (lo_a = lo_b = 0), so a slot sweeps all n_r references (a start at r0 costs this kernel spills on sm_90a).
  *   threshold: two 8-bit histogram passes find the score T of the k-th best hit;
  *   ordered pass: in reference order, every hit above T and the first (k - hits above T) hits at T become candidates;
  *   the <= k candidates are sorted in shared memory and their records written. */
 __global__ void __launch_bounds__(SSW_SELECT_THREADS)
-ssw_grid_select_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGridQ* __restrict__ qt,
+ssw_grid_select_kernel(SswGridArgs A, const SswGridQp* __restrict__ qp, const SswGridQ* __restrict__ qt,
                        const SswFillResult* __restrict__ res, int32_t k, int32_t min_score,
                        int32_t* __restrict__ hit_ref, ssw_batch_result* __restrict__ hits, int32_t* __restrict__ n_hits,
                        int32_t* __restrict__ redo_list, int32_t* __restrict__ redo_count, int32_t redo_cap)
@@ -166,14 +199,12 @@ ssw_grid_select_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGrid
 	__shared__ int32_t s_warp[2][SSW_SELECT_THREADS / 32];
 	__shared__ int32_t s_cut[3];                       /* threshold score, hits above it, hits in all */
 	__shared__ uint64_t s_key[SSW_SEARCH_MAX_K];
-	const int h = (int)(blockIdx.x & 1), pi = (int)(blockIdx.x >> 1);
-	const int2 pr = qp[pi];
-	const int q = h ? pr.y : pr.x;
+	const SswGridSlot sl = ssw_grid_slot(A.n_r, qp, qt, res);
+	const int q = sl.q;
 	if (q < 0) return;                                 /* the whole CTA: no second query in this pair-task */
-	const int mask_len = qt[q].mask_len;
-	const int n_r = A.n_r, tid = threadIdx.x;
-	const SswFillResult* rq = res + (int64_t)pi * n_r * 2 + h;       /* result of reference r: rq[2 * r] */
-	const int64_t p0 = (int64_t)q * n_r;
+	const int mask_len = sl.mask_len, n_r = A.n_r, tid = threadIdx.x;
+	const SswFillResult* rq = sl.rq;
+	const int64_t p0 = sl.p0;
 
 	/* pass 1: histogram of the high score bytes of the hits (and the redo queue) */
 	for (int i = tid; i < 256; i += SSW_SELECT_THREADS) s_hist[i] = 0;
@@ -271,15 +302,13 @@ ssw_grid_select_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGrid
  * running row, so the keys are distinct and the result is the selection over the union (grid hits never have status 1).
  * Output i comes from the merge path: x entries of the running row and i - x of the tile row precede it. */
 __global__ void __launch_bounds__(SSW_SELECT_THREADS)
-ssw_grid_merge_kernel(const int2* __restrict__ qp, int32_t k, int32_t r_base,
+ssw_grid_merge_kernel(const SswGridQp* __restrict__ qp, int32_t k, int32_t r_base,
                       int32_t* __restrict__ hit_ref, ssw_batch_result* __restrict__ hits, int32_t* __restrict__ n_hits,
                       const int32_t* __restrict__ t_ref, const ssw_batch_result* __restrict__ t_hits, const int32_t* __restrict__ t_n)
 {
 	constexpr int kPer = SSW_SEARCH_MAX_K / SSW_SELECT_THREADS;      /* outputs per thread */
 	__shared__ uint64_t s_a[SSW_SEARCH_MAX_K], s_b[SSW_SEARCH_MAX_K];
-	const int h = (int)(blockIdx.x & 1), pi = (int)(blockIdx.x >> 1);
-	const int2 pr = qp[pi];
-	const int q = h ? pr.y : pr.x;
+	const int q = blockIdx.x & 1 ? qp[blockIdx.x >> 1].qb : qp[blockIdx.x >> 1].qa;
 	if (q < 0) return;                                 /* the whole CTA: no second query in this pair-task */
 	const int tid = threadIdx.x;
 	const int64_t row = (int64_t)q * k;
@@ -319,29 +348,23 @@ ssw_grid_merge_kernel(const int2* __restrict__ qp, int32_t k, int32_t r_base,
  * that query among the group's resolve results (0 for a slot without a query).  The only kernel of the threshold search that
  * queues redo pairs: each pair of the group is visited once, so each is queued once. */
 __global__ void __launch_bounds__(SSW_SELECT_THREADS)
-ssw_grid_count_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGridQ* __restrict__ qt,
+ssw_grid_count_kernel(SswGridArgs A, const SswGridQp* __restrict__ qp, const SswGridQ* __restrict__ qt,
                       const SswFillResult* __restrict__ res, int32_t min_score, int32_t* __restrict__ slot_n,
                       int32_t* __restrict__ redo_list, int32_t* __restrict__ redo_count, int32_t redo_cap)
 {
 	__shared__ int32_t s_n;
-	const int h = (int)(blockIdx.x & 1), pi = (int)(blockIdx.x >> 1);
-	const int2 pr = qp[pi];
-	const int q = h ? pr.y : pr.x;
+	const SswGridSlot sl = ssw_grid_slot(A.n_r, qp, qt, res);
 	const int tid = threadIdx.x;
-	if (q < 0) {                                       /* the whole CTA: no second query in this pair-task */
+	if (sl.q < 0) {                                    /* the whole CTA: no second query in this pair-task */
 		if (tid == 0) slot_n[blockIdx.x] = 0;
 		return;
 	}
-	const int mask_len = qt[q].mask_len;
-	const int n_r = A.n_r;
-	const SswFillResult* rq = res + (int64_t)pi * n_r * 2 + h;
-	const int64_t p0 = (int64_t)q * n_r;
 	if (tid == 0) s_n = 0;
 	__syncthreads();
 	int c = 0;
-	for (int r = tid; r < n_r; r += SSW_SELECT_THREADS) {
+	for (int r = sl.r0 + tid; r < A.n_r; r += SSW_SELECT_THREADS) {
 		ssw_batch_result o;
-		if (ssw_grid_record<true>(rq[2 * (int64_t)r], mask_len, p0 + r, o, redo_list, redo_count, redo_cap) && o.score1 >= min_score) ++c;
+		if (ssw_grid_record<true>(sl.rq[2 * (int64_t)r], sl.mask_len, sl.p0 + r, o, redo_list, redo_count, redo_cap) && o.score1 >= min_score) ++c;
 	}
 	if (c) atomicAdd(&s_n, c);
 	__syncthreads();
@@ -352,140 +375,21 @@ ssw_grid_count_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGridQ
  * the counts over the group's slots): one ordered ballot pass, as pass 3 of the selection kernel, which stops once the slot's
  * count is reached.  Records and device reference numbers. */
 __global__ void __launch_bounds__(SSW_SELECT_THREADS)
-ssw_grid_compact_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGridQ* __restrict__ qt,
+ssw_grid_compact_kernel(SswGridArgs A, const SswGridQp* __restrict__ qp, const SswGridQ* __restrict__ qt,
                         const SswFillResult* __restrict__ res, int32_t min_score, const int64_t* __restrict__ slot_off,
                         int32_t* __restrict__ hit_ref, ssw_batch_result* __restrict__ hits)
 {
 	__shared__ int32_t s_warp[2][SSW_SELECT_THREADS / 32];
-	const int h = (int)(blockIdx.x & 1), pi = (int)(blockIdx.x >> 1);
-	const int2 pr = qp[pi];
-	const int q = h ? pr.y : pr.x;
-	if (q < 0) return;
-	const int mask_len = qt[q].mask_len;
+	const SswGridSlot sl = ssw_grid_slot(A.n_r, qp, qt, res);
+	if (sl.q < 0) return;
 	const int n_r = A.n_r, tid = threadIdx.x;
-	const SswFillResult* rq = res + (int64_t)pi * n_r * 2 + h;
-	const int64_t p0 = (int64_t)q * n_r;
 	const int64_t base = slot_off[blockIdx.x], cnt = slot_off[blockIdx.x + 1] - base;
 	int64_t done = 0;
 	/* two prefix buffers in turn: a step's writes to one cannot race the reads of the step before, which a barrier separates */
-	for (int r0 = 0, it = 0; r0 < n_r && done < cnt; r0 += SSW_SELECT_THREADS, ++it) {
-		const int r = r0 + tid;
+	for (int rb = sl.r0, it = 0; rb < n_r && done < cnt; rb += SSW_SELECT_THREADS, ++it) {
+		const int r = rb + tid;
 		ssw_batch_result o;
-		const bool hit = r < n_r && ssw_grid_record<false>(rq[2 * (int64_t)r], mask_len, p0 + r, o, nullptr, nullptr, 0) && o.score1 >= min_score;
-		int n = 0;
-		const int at = ssw_block_prefix(hit, s_warp[it & 1], &n);
-		if (hit) {
-			hits[base + done + at] = o;
-			hit_ref[base + done + at] = r;
-		}
-		done += n;
-	}
-}
-
-/* ---- self-search (ssw_engine_search_self): the pairs of one set above the diagonal of its canonical order -------------- */
-
-/* One query pair of a self-search launch.  The device numbers the tile's references in canonical order (length, then index,
- * ascending) and slot rr of every query pair sweeps reference n_r - 1 - rr (longest first).  Half a needs the references
- * [lo_a, n_r) -- those ranked after its query, the live slots [0, n_r - lo_a) -- and half b, the later query of the pair,
- * [lo_b, n_r) with lo_b >= lo_a.  Items, descriptors (two per live slot, at desc0 + r - lo_a) and column maxima (cm0 +
- * cm_prefix[r] - cm_prefix[lo_a]) are ragged: item0 is the launch's prefix of the live slots, each query pair's padded to
- * whole CTAs, and entry n_qp of the table holds the launch's item count. */
-struct SswGridSelfQp { int64_t item0, desc0, cm0; int32_t lo_a, lo_b; };
-
-/* thread idx -> item (query pair found by binary search over item0, slot rr): as ssw_grid_plan_kernel over the live slots */
-__global__ void __launch_bounds__(256)
-ssw_grid_self_plan_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGridSelfQp* __restrict__ sq, const SswGridQ* __restrict__ qt,
-                          const int64_t* __restrict__ ref_off, const int32_t* __restrict__ ref_len, const int64_t* __restrict__ cm_prefix,
-                          SswItem* __restrict__ items, SswAlnDesc* __restrict__ descs)
-{
-	const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-	if (idx >= sq[A.n_qp].item0) return;
-	int pi = 0;
-	for (int hi = A.n_qp - 1; pi < hi;) {
-		const int m = (pi + hi + 1) >> 1;
-		if (sq[m].item0 <= idx) pi = m; else hi = m - 1;
-	}
-	const SswGridSelfQp s = sq[pi];
-	const int rr = (int)(idx - s.item0);
-	const bool live = rr < A.n_r - s.lo_a;
-	const int r = A.n_r - 1 - (live ? rr : 0);
-	const int2 pr = qp[pi];
-	const SswGridQ qa = qt[pr.x];
-	SswItem it;
-	it.qa.off = qa.off; it.qa.len = qa.len; it.qa.lp = qa.lp; it.qa.rev = 0;
-	it.qb.off = 0; it.qb.len = 0; it.qb.lp = 0; it.qb.rev = 0;
-	SswGridQ qb;
-	qb.off = 0; qb.len = 0; qb.lp = 0; qb.mask_len = 0; qb.limit = 0;
-	if (pr.y >= 0) { qb = qt[pr.y]; it.qb.off = qb.off; it.qb.len = qb.len; it.qb.lp = qb.lp; }
-	it.ref_off = ref_off[r]; it.ref_len = ref_len[r];
-	it.cend = (A.arm_tail > 0 && live) ? max(0, ref_len[r] - A.arm_tail) : 0;
-	it.p0 = 0; it.p1 = live ? ref_len[r] : 0; it.warm = 0; it.term_a = -1;
-	it.cm_off = live ? s.cm0 + cm_prefix[r] - cm_prefix[s.lo_a] : SSW_CM_NONE;
-	items[idx] = it;
-	if (live) {
-		SswAlnDesc d;
-		d.first_item = (int32_t)idx; d.n_items = 1; d.half = 0; d.ref_len = it.ref_len; d.read_len = qa.len;
-		d.word = A.word; d.limit = qa.limit; d.mask_len = qa.mask_len; d.cm_off = it.cm_off; d.scan_all = 0; d.warm = 0; d.byte_pad = 0;
-		const int64_t di = (s.desc0 + r - s.lo_a) * 2;
-		descs[di] = d;
-		d.half = 1; d.read_len = qb.len; d.mask_len = qb.mask_len; d.limit = qb.limit;
-		if (pr.y < 0 || r < s.lo_b) d.n_items = 0;                     /* no second query, or not ranked after it: skipped */
-		descs[di + 1] = d;
-	}
-}
-
-/* ssw_grid_count_kernel over the references of the slot's half only: [lo_a, n_r) or [lo_b, n_r) */
-__global__ void __launch_bounds__(SSW_SELECT_THREADS)
-ssw_grid_self_count_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGridSelfQp* __restrict__ sq, const SswGridQ* __restrict__ qt,
-                           const SswFillResult* __restrict__ res, int32_t min_score, int32_t* __restrict__ slot_n,
-                           int32_t* __restrict__ redo_list, int32_t* __restrict__ redo_count, int32_t redo_cap)
-{
-	__shared__ int32_t s_n;
-	const int h = (int)(blockIdx.x & 1), pi = (int)(blockIdx.x >> 1);
-	const int2 pr = qp[pi];
-	const int q = h ? pr.y : pr.x;
-	const int tid = threadIdx.x;
-	if (q < 0) {
-		if (tid == 0) slot_n[blockIdx.x] = 0;
-		return;
-	}
-	const SswGridSelfQp s = sq[pi];
-	const int mask_len = qt[q].mask_len;
-	const int n_r = A.n_r;
-	const int64_t d0 = s.desc0 - s.lo_a, p0 = (int64_t)q * n_r;          /* result of reference r: res[2 * (d0 + r) + h] */
-	if (tid == 0) s_n = 0;
-	__syncthreads();
-	int c = 0;
-	for (int r = (h ? s.lo_b : s.lo_a) + tid; r < n_r; r += SSW_SELECT_THREADS) {
-		ssw_batch_result o;
-		if (ssw_grid_record<true>(res[2 * (d0 + r) + h], mask_len, p0 + r, o, redo_list, redo_count, redo_cap) && o.score1 >= min_score) ++c;
-	}
-	if (c) atomicAdd(&s_n, c);
-	__syncthreads();
-	if (tid == 0) slot_n[blockIdx.x] = s_n;
-}
-
-/* ssw_grid_compact_kernel over the same references */
-__global__ void __launch_bounds__(SSW_SELECT_THREADS)
-ssw_grid_self_compact_kernel(SswGridArgs A, const int2* __restrict__ qp, const SswGridSelfQp* __restrict__ sq, const SswGridQ* __restrict__ qt,
-                             const SswFillResult* __restrict__ res, int32_t min_score, const int64_t* __restrict__ slot_off,
-                             int32_t* __restrict__ hit_ref, ssw_batch_result* __restrict__ hits)
-{
-	__shared__ int32_t s_warp[2][SSW_SELECT_THREADS / 32];
-	const int h = (int)(blockIdx.x & 1), pi = (int)(blockIdx.x >> 1);
-	const int2 pr = qp[pi];
-	const int q = h ? pr.y : pr.x;
-	if (q < 0) return;
-	const SswGridSelfQp s = sq[pi];
-	const int mask_len = qt[q].mask_len;
-	const int n_r = A.n_r, tid = threadIdx.x;
-	const int64_t d0 = s.desc0 - s.lo_a, p0 = (int64_t)q * n_r;
-	const int64_t base = slot_off[blockIdx.x], cnt = slot_off[blockIdx.x + 1] - base;
-	int64_t done = 0;
-	for (int r0 = h ? s.lo_b : s.lo_a, it = 0; r0 < n_r && done < cnt; r0 += SSW_SELECT_THREADS, ++it) {
-		const int r = r0 + tid;
-		ssw_batch_result o;
-		const bool hit = r < n_r && ssw_grid_record<false>(res[2 * (d0 + r) + h], mask_len, p0 + r, o, nullptr, nullptr, 0) && o.score1 >= min_score;
+		const bool hit = r < n_r && ssw_grid_record<false>(sl.rq[2 * (int64_t)r], sl.mask_len, sl.p0 + r, o, nullptr, nullptr, 0) && o.score1 >= min_score;
 		int n = 0;
 		const int at = ssw_block_prefix(hit, s_warp[it & 1], &n);
 		if (hit) {

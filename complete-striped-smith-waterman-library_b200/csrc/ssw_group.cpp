@@ -158,6 +158,68 @@ inline int64_t global_pair(const Job& J, const Shard& S, int64_t l)
 	return l < plus ? (int64_t)S.q0 * J.n_r + l : ((int64_t)J.n_q + S.q0) * J.n_r + (l - plus);
 }
 
+/* work(d) for every device d of the group: one host thread per device, the calling thread taking device 0 */
+template <class F> void for_each_device(const ssw_group* g, const F& work)
+{
+	const int world = (int)g->eng.size();
+#ifdef SSW_CPU_EMU
+	for (int d = 0; d < world; ++d) work(d);        /* the emulator's fibers are not thread-safe */
+#else
+	std::vector<std::thread> th;
+	th.reserve((size_t)world);
+	for (int d = 1; d < world; ++d) {
+		try { th.emplace_back([&work, d] { work(d); }); }
+		catch (...) { work(d); }                     /* no thread to be had: this block runs here */
+	}
+	work(0);
+	for (std::thread& t : th) t.join();
+#endif
+}
+
+/* one device's hit set (ssw_engine_search_all, ssw_engine_search_self) and return code */
+struct HitPart {
+	ssw_hit_set* set = nullptr;
+	int rc = 0;
+	HitPart() = default;
+	HitPart(const HitPart&) = delete;
+	HitPart& operator=(const HitPart&) = delete;
+	~HitPart() { ssw_hit_set_destroy(set); }
+};
+
+/* The hit set of a device group from the sets of its devices: row i is row rows[i].second of device rows[i].first's set, and the
+ * CIGAR pools are concatenated in device order with every offset re-based.  Returns -2 (`fn` says so) above max_hits hits. */
+int gather_hits(const char* fn, const std::vector<HitPart>& parts, const std::vector<std::pair<int, int32_t>>& rows,
+                int64_t max_hits, ssw_hit_set** out)
+{
+	int64_t n_hits = 0, n_words = 0;
+	for (const HitPart& S : parts) if (S.set) { n_hits += (int64_t)S.set->hits.size(); n_words += (int64_t)S.set->pool.size(); }
+	if (n_hits > max_hits) { fprintf(stderr, "[libssw-b200] %s: more than max_hits = %lld hits\n", fn, (long long)max_hits); return -2; }
+	if (n_words > 0x7fffffff) { fprintf(stderr, "[libssw-b200] more than 2^31 CIGAR words in one batch: split the batch\n"); return -1; }
+	std::unique_ptr<ssw_hit_set> s(new ssw_hit_set());
+	s->n_rows = (int32_t)rows.size();
+	s->row_off.reserve(rows.size() + 1);
+	s->row_off.push_back(0);
+	s->hit_ref.reserve((size_t)n_hits); s->hits.reserve((size_t)n_hits); s->pool.reserve((size_t)n_words);
+	std::vector<int64_t> base(parts.size(), 0);
+	for (size_t d = 0; d < parts.size(); ++d) {
+		if (!parts[d].set) continue;
+		base[d] = (int64_t)s->pool.size();
+		s->pool.insert(s->pool.end(), parts[d].set->pool.begin(), parts[d].set->pool.end());
+	}
+	for (const std::pair<int, int32_t>& row : rows) {
+		const ssw_hit_set& S = *parts[row.first].set;
+		for (int64_t i = S.row_off[row.second]; i < S.row_off[row.second + 1]; ++i) {
+			ssw_batch_result o = S.hits[i];
+			if (o.cigar_off >= 0) o.cigar_off += (int32_t)base[row.first];
+			s->hits.push_back(o);
+			s->hit_ref.push_back(S.hit_ref[i]);
+		}
+		s->row_off.push_back((int64_t)s->hits.size());
+	}
+	*out = s.release();
+	return 0;
+}
+
 int run_job(ssw_group* g, const Job& J, std::vector<Shard>& shards, ssw_batch_result* results)
 {
 	const ssw_batch_params& P = *J.P;
@@ -195,20 +257,7 @@ int run_job(ssw_group* g, const Job& J, std::vector<Shard>& shards, ssw_batch_re
 		});
 		for (int d = 0; d < world; ++d) { shards[d].p0 = b[d]; shards[d].p1 = b[d + 1]; if (results) shards[d].ext = results + b[d]; }
 	}
-#ifdef SSW_CPU_EMU
-	for (int d = 0; d < world; ++d) run_shard(g->eng[d], JJ, shards[d]);        /* the emulator's fibers are not thread-safe */
-#else
-	{
-		std::vector<std::thread> th;
-		th.reserve((size_t)world);
-		for (int d = 1; d < world; ++d) {
-			try { th.emplace_back([&, d] { run_shard(g->eng[d], JJ, shards[d]); }); }
-			catch (...) { run_shard(g->eng[d], JJ, shards[d]); }       /* no thread to be had: this block runs here */
-		}
-		run_shard(g->eng[0], JJ, shards[0]);
-		for (std::thread& t : th) t.join();
-	}
-#endif
+	for_each_device(g, [&](int d) { run_shard(g->eng[d], JJ, shards[d]); });
 	for (const Shard& S : shards) if (S.rc) return S.rc;
 	return 0;
 }
@@ -346,20 +395,7 @@ extern "C" int ssw_group_search(ssw_group* g, const ssw_batch_params* params, co
 			catch (const std::exception& ex) { fprintf(stderr, "[libssw-b200] device group: %s\n", ex.what()); S.rc = -1; }
 			catch (...) { S.rc = -1; }
 		};
-#ifdef SSW_CPU_EMU
-		for (int d = 0; d < world; ++d) work(d);        /* the emulator's fibers are not thread-safe */
-#else
-		{
-			std::vector<std::thread> th;
-			th.reserve((size_t)world);
-			for (int d = 1; d < world; ++d) {
-				try { th.emplace_back(work, d); }
-				catch (...) { work(d); }                 /* no thread to be had: this block runs here */
-			}
-			work(0);
-			for (std::thread& t : th) t.join();
-		}
-#endif
+		for_each_device(g, work);
 		for (const Part& S : parts) if (S.rc) return S.rc;
 		int64_t base = 0;
 		for (const Part& S : parts) {
@@ -398,15 +434,6 @@ extern "C" int ssw_group_search_all(ssw_group* g, const ssw_batch_params* params
 	if (!g || g->eng.empty() || !params || !params->mat) { fprintf(stderr, "[libssw-b200] ssw_group_search_all: NULL argument\n"); return -1; }
 	if (max_hits < 0) { fprintf(stderr, "[libssw-b200] ssw_group_search_all: max_hits = %lld is negative\n", (long long)max_hits); return -1; }
 	if (n_queries <= 0 || n_refs <= 0 || !queries || !refs || !query_off || !ref_off) { fprintf(stderr, "[libssw-b200] ssw_group_search_all: no sequences\n"); return -1; }
-	struct Part {
-		int32_t q0 = 0, nq = 0;      /* first query and queries of the block; its set has nq (or 2 nq) rows */
-		ssw_hit_set* set = nullptr;
-		int rc = 0;
-		Part() = default;
-		Part(const Part&) = delete;
-		Part& operator=(const Part&) = delete;
-		~Part() { ssw_hit_set_destroy(set); }
-	};
 	try {
 		const ssw_batch_params& P = *params;
 		for (int32_t q = 0; q < n_queries; ++q) if (query_off[q + 1] < query_off[q]) { fprintf(stderr, "[libssw-b200] query offsets are not non-decreasing at %d\n", q); return -1; }
@@ -415,72 +442,35 @@ extern "C" int ssw_group_search_all(ssw_group* g, const ssw_batch_params* params
 		/* the queries cut as for ssw_group_search; every device searches its block against all references */
 		const int world = (int)g->eng.size();
 		const std::vector<int64_t> b = balanced_bounds(n_queries, world, [&](int64_t q) { return query_off[q + 1] - query_off[q] + 1; });
-		std::vector<Part> parts((size_t)world);
+		std::vector<HitPart> parts((size_t)world);
 		auto work = [&](int d) {
-			Part& S = parts[d];
+			HitPart& S = parts[d];
 			try {
-				S.q0 = (int32_t)b[d];
-				S.nq = (int32_t)(b[d + 1] - b[d]);
-				if (S.nq <= 0) return;
-				std::vector<int64_t> qoff((size_t)S.nq + 1);
-				for (int32_t j = 0; j <= S.nq; ++j) qoff[j] = query_off[S.q0 + j] - query_off[S.q0];
-				const char* qbase = (const char*)queries + query_off[S.q0];
+				const int32_t q0 = (int32_t)b[d], nq = (int32_t)(b[d + 1] - b[d]);
+				if (nq <= 0) return;
+				std::vector<int64_t> qoff((size_t)nq + 1);
+				for (int32_t j = 0; j <= nq; ++j) qoff[j] = query_off[q0 + j] - query_off[q0];
+				const char* qbase = (const char*)queries + query_off[q0];
 				ssw_engine* e = g->eng[d];
-				S.rc = table ? ssw_engine_set_sequences_text(e, S.nq, qbase, qoff.data(), n_refs, (const char*)refs, ref_off, table, P.n, add_rc ? 1 : 0)
-				             : ssw_engine_set_sequences(e, S.nq, (const int8_t*)qbase, qoff.data(), n_refs, (const int8_t*)refs, ref_off);
+				S.rc = table ? ssw_engine_set_sequences_text(e, nq, qbase, qoff.data(), n_refs, (const char*)refs, ref_off, table, P.n, add_rc ? 1 : 0)
+				             : ssw_engine_set_sequences(e, nq, (const int8_t*)qbase, qoff.data(), n_refs, (const int8_t*)refs, ref_off);
 				if (S.rc) return;
 				S.rc = ssw_engine_search_all(e, &P, min_score, max_hits, &S.set);      /* each block alone is bounded by the total's bound */
 			}
 			catch (const std::exception& ex) { fprintf(stderr, "[libssw-b200] device group: %s\n", ex.what()); S.rc = -1; }
 			catch (...) { S.rc = -1; }
 		};
-#ifdef SSW_CPU_EMU
-		for (int d = 0; d < world; ++d) work(d);        /* the emulator's fibers are not thread-safe */
-#else
-		{
-			std::vector<std::thread> th;
-			th.reserve((size_t)world);
-			for (int d = 1; d < world; ++d) {
-				try { th.emplace_back(work, d); }
-				catch (...) { work(d); }                 /* no thread to be had: this block runs here */
-			}
-			work(0);
-			for (std::thread& t : th) t.join();
-		}
-#endif
-		for (const Part& S : parts) if (S.rc) return S.rc;
-		int64_t n_hits = 0, n_words = 0;
-		for (const Part& S : parts) if (S.set) { n_hits += (int64_t)S.set->hits.size(); n_words += (int64_t)S.set->pool.size(); }
-		if (n_hits > max_hits) { fprintf(stderr, "[libssw-b200] ssw_group_search_all: more than max_hits = %lld hits\n", (long long)max_hits); return -2; }
-		if (n_words > 0x7fffffff) { fprintf(stderr, "[libssw-b200] more than 2^31 CIGAR words in one batch: split the batch\n"); return -1; }
+		for_each_device(g, work);
+		for (const HitPart& S : parts) if (S.rc) return S.rc;
 		/* rows in query order -- every block's queries, then (reverse complements) every block's second half -- keep pair order */
-		std::unique_ptr<ssw_hit_set> s(new ssw_hit_set());
-		s->n_rows = n_queries * (add_rc ? 2 : 1);
-		s->row_off.reserve((size_t)s->n_rows + 1);
-		s->row_off.push_back(0);
-		s->hit_ref.reserve((size_t)n_hits); s->hits.reserve((size_t)n_hits); s->pool.reserve((size_t)n_words);
-		std::vector<int64_t> base((size_t)world, 0);
-		for (int d = 0; d < world; ++d) {
-			if (!parts[d].set) continue;
-			base[d] = (int64_t)s->pool.size();
-			s->pool.insert(s->pool.end(), parts[d].set->pool.begin(), parts[d].set->pool.end());
-		}
+		std::vector<std::pair<int, int32_t>> rows;
+		rows.reserve((size_t)n_queries * (add_rc ? 2 : 1));
 		for (int half = 0; half < (add_rc ? 2 : 1); ++half)
 			for (int d = 0; d < world; ++d) {
-				const Part& S = parts[d];
-				if (!S.set) continue;
-				for (int32_t l = half * S.nq; l < (half + 1) * S.nq; ++l) {
-					for (int64_t i = S.set->row_off[l]; i < S.set->row_off[l + 1]; ++i) {
-						ssw_batch_result o = S.set->hits[i];
-						if (o.cigar_off >= 0) o.cigar_off += (int32_t)base[d];
-						s->hits.push_back(o);
-						s->hit_ref.push_back(S.set->hit_ref[i]);
-					}
-					s->row_off.push_back((int64_t)s->hits.size());
-				}
+				const int32_t nq = (int32_t)(b[d + 1] - b[d]);
+				for (int32_t l = half * nq; l < (half + 1) * nq; ++l) rows.emplace_back(d, l);
 			}
-		*out = s.release();
-		return 0;
+		return gather_hits("ssw_group_search_all", parts, rows, max_hits, out);
 	}
 	catch (const std::exception& ex) { fprintf(stderr, "[libssw-b200] ssw_group_search_all: %s\n", ex.what()); return -1; }
 	catch (...) { return -1; }
@@ -493,14 +483,6 @@ extern "C" int ssw_group_search_self(ssw_group* g, const ssw_batch_params* param
 	*out = nullptr;
 	if (!g || g->eng.empty() || !params) { fprintf(stderr, "[libssw-b200] ssw_group_search_self: NULL argument\n"); return -1; }
 	if (n < 0 || (n > 0 && (!seqs || !off))) { fprintf(stderr, "[libssw-b200] ssw_group_search_self: no sequences\n"); return -1; }
-	struct Part {
-		ssw_hit_set* set = nullptr;
-		int rc = 0;
-		Part() = default;
-		Part(const Part&) = delete;
-		Part& operator=(const Part&) = delete;
-		~Part() { ssw_hit_set_destroy(set); }
-	};
 	try {
 		for (int32_t i = 0; i < n; ++i) if (off[i + 1] < off[i]) { fprintf(stderr, "[libssw-b200] offsets are not non-decreasing at %d\n", i); return -1; }
 		/* canonical order (length, then index) and the triangle cells of each rank: its length times the letters ranked after it */
@@ -514,9 +496,9 @@ extern "C" int ssw_group_search_self(ssw_group* g, const ssw_batch_params* param
 		for (int32_t t = n - 1; t >= 0; --t) { cells[t] = (long double)len(canon[t]) * later; later += len(canon[t]); }
 		const int world = (int)g->eng.size();
 		const std::vector<int64_t> b = balanced_bounds(n, world, [&](int64_t t) { return cells[t]; });
-		std::vector<Part> parts((size_t)world);
+		std::vector<HitPart> parts((size_t)world);
 		auto work = [&](int d) {
-			Part& S = parts[d];
+			HitPart& S = parts[d];
 			try {
 				ssw_engine* e = g->eng[d];
 				S.rc = ssw_engine_set_sequences_self(e, n, seqs, off);
@@ -526,49 +508,12 @@ extern "C" int ssw_group_search_self(ssw_group* g, const ssw_batch_params* param
 			catch (const std::exception& ex) { fprintf(stderr, "[libssw-b200] device group: %s\n", ex.what()); S.rc = -1; }
 			catch (...) { S.rc = -1; }
 		};
-#ifdef SSW_CPU_EMU
-		for (int d = 0; d < world; ++d) work(d);        /* the emulator's fibers are not thread-safe */
-#else
-		{
-			std::vector<std::thread> th;
-			th.reserve((size_t)world);
-			for (int d = 1; d < world; ++d) {
-				try { th.emplace_back(work, d); }
-				catch (...) { work(d); }
-			}
-			work(0);
-			for (std::thread& t : th) t.join();
-		}
-#endif
-		for (const Part& S : parts) if (S.rc) return S.rc;
-		int64_t n_hits = 0, n_words = 0;
-		for (const Part& S : parts) { n_hits += (int64_t)S.set->hits.size(); n_words += (int64_t)S.set->pool.size(); }
-		if (n_hits > max_hits) { fprintf(stderr, "[libssw-b200] ssw_group_search_self: more than max_hits = %lld hits\n", (long long)max_hits); return -2; }
-		if (n_words > 0x7fffffff) { fprintf(stderr, "[libssw-b200] more than 2^31 CIGAR words in one batch: split the batch\n"); return -1; }
+		for_each_device(g, work);
+		for (const HitPart& S : parts) if (S.rc) return S.rc;
 		/* row i comes from the device whose rank range holds rank[i] */
-		std::unique_ptr<ssw_hit_set> s(new ssw_hit_set());
-		s->n_rows = n;
-		s->row_off.reserve((size_t)n + 1);
-		s->row_off.push_back(0);
-		s->hit_ref.reserve((size_t)n_hits); s->hits.reserve((size_t)n_hits); s->pool.reserve((size_t)n_words);
-		std::vector<int64_t> base((size_t)world, 0);
-		for (int d = 0; d < world; ++d) {
-			base[d] = (int64_t)s->pool.size();
-			s->pool.insert(s->pool.end(), parts[d].set->pool.begin(), parts[d].set->pool.end());
-		}
-		for (int32_t i = 0; i < n; ++i) {
-			const int d = (int)(std::upper_bound(b.begin(), b.end(), (int64_t)rank[i]) - b.begin()) - 1;
-			const ssw_hit_set& S = *parts[d].set;
-			for (int64_t j = S.row_off[i]; j < S.row_off[i + 1]; ++j) {
-				ssw_batch_result o = S.hits[j];
-				if (o.cigar_off >= 0) o.cigar_off += (int32_t)base[d];
-				s->hits.push_back(o);
-				s->hit_ref.push_back(S.hit_ref[j]);
-			}
-			s->row_off.push_back((int64_t)s->hits.size());
-		}
-		*out = s.release();
-		return 0;
+		std::vector<std::pair<int, int32_t>> rows((size_t)n);
+		for (int32_t i = 0; i < n; ++i) rows[i] = {(int)(std::upper_bound(b.begin(), b.end(), (int64_t)rank[i]) - b.begin()) - 1, i};
+		return gather_hits("ssw_group_search_self", parts, rows, max_hits, out);
 	}
 	catch (const std::exception& ex) { fprintf(stderr, "[libssw-b200] ssw_group_search_self: %s\n", ex.what()); return -1; }
 	catch (...) { return -1; }
